@@ -365,9 +365,10 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
 // candidate length and the cheapest wins.
 struct SlidePlan { int chunks, cvc, seg_rows, groups, gy; };
 
-inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, int K, int ctas_per_sm, bool per_sample) {
+inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, int K, int ctas_per_sm, bool per_sample,
+                            int cvc_cap = kST) {
   SlidePlan pl;
-  const int cvc_max = kChMax / V < kST ? kChMax / V : kST;
+  const int cvc_max = min(kChMax / V < kST ? kChMax / V : kST, cvc_cap);
   pl.chunks = ceil_div(cv, cvc_max);
   pl.cvc = ceil_div(cv, pl.chunks);
   const int ppb = kST / pl.cvc > 0 ? kST / pl.cvc : 1;
@@ -1080,7 +1081,431 @@ int launch_dg2_slide(Dg2Args a, int k, cudaStream_t st) {
   return EAT_OK;
 }
 
+
+// ------------------------------------------------------------------------------------------ fused depthwise backward
+// The whole backward of a depthwise stage whose raw output z2 feeds a BatchNorm + activation (BN2), in one walk:
+//   dz   = BN2-backward apply of (dp, z2): scale2 * g * act'(z2*scale2+shift2) + alpha * z2 + beta, g = dp*gate + dpool
+//          (the constants of bn_bwd_apply2_kernel), computed as each dz element is loaded and never stored
+//   din  = depthwise data gradient of dz (+ res), stored
+//   dW  += sum dz * xf(in),  xf = act(in*in_scale+in_shift) (the expand stage's BatchNorm + activation) or identity
+//   s1  += sum g1, s2 += invstd1 * sum g1*(in-mean1),  g1 = din * act'(in*in_scale+in_shift)  (optional: the expand
+//          BatchNorm's backward reduce, what eat_bn_bwd_reduce(gA = din) yields)
+// The data and the weight gradient visit the same (din element, dz element, tap) triples, so both come out of a walk
+// organised by din elements, as dw_dgrad2_slide_kernel: a thread owns a channel vector and Q din columns, walks down its
+// segment (single din rows for stride 1, row pairs for stride 2) and keeps the LW dz rows they read in a register
+// window.  Per step ONE cp.async group brings the new dz row (dp and z2 over the strip and its halo) and the step's S input
+// rows (own columns only) into the thread's ring slot, two steps ahead.
+// Algorithmic bytes: dp, z2, in read once, din written once (2*T2 + 2*T1 elements); the separate passes (BN2 apply,
+// weight gradient, data gradient, BN1 reduce) move 5*T2 + 4*T1.
+struct FusedBwdArgs {
+  const float* dp;
+  const float* gate;
+  const float* dpool;
+  const float* z2;
+  const float* scale;
+  const float* shift;
+  const float* mean;
+  const float* invstd;
+  const float* c1;
+  const float* c2;
+  const float* wt;
+  const float* in;
+  const float* in_scale;
+  const float* in_shift;
+  const float* res;
+  float* din;
+  float* dw;
+  const float* zmean;
+  const float* zinvstd;
+  double* s1;
+  double* s2;
+  int B, F, Tn, Fo, To, C;
+  int cvc, chunks, seg_rows;   // seg_rows counts steps (din rows for stride 1, row pairs for stride 2)
+};
+
+template <int V> struct VecF;
+template <> struct VecF<4> {
+  __device__ __forceinline__ static void load(const float* p, float (&v)[4]) { Vec<float>::load(p, v); }
+  __device__ __forceinline__ static void store(float* p, const float (&v)[4]) { Vec<float>::store(p, v); }
+};
+template <> struct VecF<2> {
+  __device__ __forceinline__ static void load(const float* p, float (&v)[2]) {
+    const float2 t = *reinterpret_cast<const float2*>(p);
+    v[0] = t.x; v[1] = t.y;
+  }
+  __device__ __forceinline__ static void store(float* p, const float (&v)[2]) {
+    *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
+  }
+};
+
+constexpr int kFbCvcMax = 32;   // channel vectors per CTA: keeps the five per-CTA tables small next to the ring
+constexpr int kFbDepth = 2;     // ring depth in steps
+
+// V: channels per thread (the 5x5 kernels keep 25 x V tap accumulators, so they take 2); Q: din columns per strip
+template <int K, int S> struct FbShape {
+  static constexpr int V = K == 3 ? 4 : 2;
+  static constexpr int Q = (S == 2 && K == 5) ? 4 : 2;
+  static constexpr int PAD = (K - 1) / 2;
+  static constexpr int LW = S == 1 ? K : (K + 1) / 2;                   // dz rows read by one step
+  static constexpr int NDZ = S == 1 ? Q + 2 * PAD : Q / 2 + PAD / 2 + 1;  // dz columns read by Q din columns
+  static constexpr int OB0 = S == 1 ? PAD : PAD / 2;                    // window slot 0 <-> dz row m - OB0
+  static constexpr int NV = 2 * NDZ + S * Q;                            // ring vectors per step: dp, z2, input rows
+  // resident CTAs per SM the register budget is planned for: 3 (<= 168 registers) fits the 3x3 stride-2 walk; the
+  // stride-1 windows (K dz rows) and the 25 tap accumulators of the 5x5 spill there, so they take 2 (<= 255 registers)
+  static constexpr int MINB = (K == 3 && S == 2) ? 3 : 2;
+};
+
+template <int K, int S, int ACT, bool XF>
+__global__ void __launch_bounds__(kST, FbShape<K, S>::MINB) dw_bwd_fused_kernel(const FusedBwdArgs a) {
+  using Sh = FbShape<K, S>;
+  constexpr int V = Sh::V, Q = Sh::Q, PAD = Sh::PAD, LW = Sh::LW, NDZ = Sh::NDZ, OB0 = Sh::OB0, NV = Sh::NV;
+  constexpr int KK = K * K, VB = V * (int)sizeof(float);
+  extern __shared__ __align__(16) float smem[];
+  const int F = a.F, Tn = a.Tn, Fo = a.Fo, To = a.To, C = a.C;
+  const int chunk = blockIdx.x % a.chunks, grp = blockIdx.x / a.chunks, groups = gridDim.x / a.chunks;
+  const int cv = C / V;
+  const int cv0 = chunk * a.cvc;
+  const int ncv = min(a.cvc, cv - cv0);
+  const int cc = ncv * V;
+  const int cst = a.cvc * V;                     // channel stride of the per-CTA tables
+  float* s_w = smem;                             // [KK][cst] taps
+  float* s_acc = s_w + KK * cst;                 // [KK][cst] weight-gradient partial sums
+  float* s_bn = s_acc + KK * cst;                // [7][cst] BN2 scale, shift, alpha, beta; xf scale, shift; BN1 mean
+  float* s_red = s_bn + 7 * cst;                 // [2][cst] BN1 partial sums
+  float* s_end = s_red + 2 * cst;                // the prefetch ring follows: [depth][NV][kST] vectors
+  const int tid = threadIdx.x;
+  const uint32_t ring0 = (uint32_t)__cvta_generic_to_shared(s_end) + (uint32_t)tid * VB;
+  const unsigned char* ringp = reinterpret_cast<const unsigned char*>(s_end) + tid * VB;
+  const bool red = XF && a.s1 != nullptr;
+  for (int i = tid; i < KK * cc; i += kST) {
+    const int tap = i / cc, c = i - tap * cc;
+    s_w[tap * cst + c] = __ldg(a.wt + (size_t)tap * C + cv0 * V + c);
+    s_acc[tap * cst + c] = 0.f;
+  }
+  for (int c = tid; c < cc; c += kST) {
+    const int cg = cv0 * V + c;
+    const float sc = __ldg(a.scale + cg);
+    const float al = -sc * __ldg(a.c2 + cg) * __ldg(a.invstd + cg);
+    s_bn[c] = sc;
+    s_bn[cst + c] = __ldg(a.shift + cg);
+    s_bn[2 * cst + c] = al;
+    s_bn[3 * cst + c] = -sc * __ldg(a.c1 + cg) - al * __ldg(a.mean + cg);
+    if (XF) {
+      s_bn[4 * cst + c] = __ldg(a.in_scale + cg);
+      s_bn[5 * cst + c] = __ldg(a.in_shift + cg);
+      s_bn[6 * cst + c] = red ? __ldg(a.zmean + cg) : 0.f;
+    }
+    s_red[c] = 0.f;
+    s_red[cst + c] = 0.f;
+  }
+  __syncthreads();
+  const int ppb = kST / ncv;
+  const int cvl = tid % ncv, slot = tid / ncv;
+  float wacc[KK][V];
+  float lsum[V], lsq[V];
+#pragma unroll
+  for (int q = 0; q < KK; ++q)
+#pragma unroll
+    for (int i = 0; i < V; ++i) wacc[q][i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < V; ++i) { lsum[i] = 0.f; lsq[i] = 0.f; }
+  if (slot < ppb) {
+    const int c0 = (cv0 + cvl) * V;
+    const float* wl = s_w + cvl * V;
+    const float* bnl = s_bn + cvl * V;
+    const int rows = S == 1 ? F : (F + 1) / 2;
+    const int strips = ceil_div(Tn, Q), segs = ceil_div(rows, a.seg_rows), units = strips * segs;
+    long long g = ((long long)blockIdx.y * groups + grp) * ppb + slot;
+    const long long gend = (long long)a.B * units;
+    const long long gstep = (long long)gridDim.y * groups * ppb;
+    for (; g < gend; g += gstep) {
+      const int b = (int)(g / units);
+      const int u = (int)(g - (long long)b * units);
+      const int seg = u / strips, strip = u - seg * strips;
+      const int m_a = seg * a.seg_rows;
+      const int nstep = min(a.seg_rows, rows - m_a);
+      const int t_a = strip * Q;                                 // even
+      const int to_base = S == 1 ? t_a - PAD : t_a / 2 - PAD / 2;  // dz column of window index 0
+      unsigned cmask = 0, qmask = 0;
+#pragma unroll
+      for (int j = 0; j < NDZ; ++j) cmask |= (to_base + j >= 0 && to_base + j < To) ? (1u << j) : 0u;
+#pragma unroll
+      for (int q = 0; q < Q; ++q) qmask |= (t_a + q < Tn) ? (1u << q) : 0u;
+      float gt[V], dpl[V];
+#pragma unroll
+      for (int i = 0; i < V; ++i) {
+        gt[i] = a.gate != nullptr ? __ldg(a.gate + (size_t)b * C + c0 + i) : 1.f;
+        dpl[i] = a.dpool != nullptr ? __ldg(a.dpool + (size_t)b * C + c0 + i) : 0.f;
+      }
+      const size_t zoff = (size_t)b * Fo * To * C + c0, ioff = (size_t)b * F * Tn * C + c0;
+      const float* dpp = a.dp + zoff + (long long)to_base * C;   // column j of dz row o: + (o * To + j) * C
+      const float* zzp = a.z2 + zoff + (long long)to_base * C;
+      const float* inp = a.in + ioff + (size_t)t_a * C;           // column q of input row i: + (i * Tn + q) * C
+      float* dinp = a.din + ioff + (size_t)t_a * C;
+      const float* resp = a.res != nullptr ? a.res + ioff + (size_t)t_a * C : nullptr;
+
+      auto dz_of = [&](const float (&p)[V], const float (&z)[V], float (&o)[V]) {
+        float sc[V], sh[V], al[V], be[V];
+        VecF<V>::load(bnl, sc);
+        VecF<V>::load(bnl + cst, sh);
+        VecF<V>::load(bnl + 2 * cst, al);
+        VecF<V>::load(bnl + 3 * cst, be);
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+          const float gg = fmaf(p[i], gt[i], dpl[i]) * act_bwd(fmaf(z[i], sc[i], sh[i]), ACT);
+          o[i] = fmaf(sc[i], gg, fmaf(al[i], z[i], be[i]));
+        }
+      };
+      auto load_dz = [&](int o, float (&dst)[NDZ][V]) {          // synchronous: the window rows before the first step
+#pragma unroll
+        for (int j = 0; j < NDZ; ++j) {
+          if (o >= 0 && o < Fo && ((cmask >> j) & 1u)) {
+            float p[V], z[V];
+            VecF<V>::load(dpp + ((size_t)o * To + j) * C, p);
+            VecF<V>::load(zzp + ((size_t)o * To + j) * C, z);
+            dz_of(p, z, dst[j]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < V; ++i) dst[j][i] = 0.f;
+          }
+        }
+      };
+      // step mm: dz row m - OB0 + LW - 1 (vectors 0 .. 2*NDZ-1: dp, z2) and input rows S*m .. S*m+S-1 (own columns)
+      auto issue = [&](int mm, int slot_) {
+        if (mm < nstep) {
+          const int m = m_a + mm;
+          const int o = m - OB0 + LW - 1;
+          const uint32_t dst = ring0 + (uint32_t)(slot_ * NV) * (kST * VB);
+          if (o >= 0 && o < Fo) {
+#pragma unroll
+            for (int j = 0; j < NDZ; ++j) {
+              if ((cmask >> j) & 1u) {
+                cp_async<VB>(dst + (uint32_t)j * (kST * VB), dpp + ((size_t)o * To + j) * C);
+                cp_async<VB>(dst + (uint32_t)(NDZ + j) * (kST * VB), zzp + ((size_t)o * To + j) * C);
+              }
+            }
+          }
+#pragma unroll
+          for (int r = 0; r < S; ++r) {
+            const int irow = S * m + r;
+            if (irow < F) {
+#pragma unroll
+              for (int q = 0; q < Q; ++q)
+                if ((qmask >> q) & 1u) cp_async<VB>(dst + (uint32_t)(2 * NDZ + r * Q + q) * (kST * VB), inp + ((size_t)irow * Tn + q) * C);
+            }
+          }
+        }
+        cp_commit();
+      };
+      auto ring = [&](int slot_, int v, float (&dst)[V]) {
+        VecF<V>::load(reinterpret_cast<const float*>(ringp + (size_t)(slot_ * NV + v) * (kST * VB)), dst);
+      };
+
+      for (int q = 0; q < kFbDepth; ++q) issue(q, q);
+      float win[LW][NDZ][V];
+#pragma unroll
+      for (int l = 1; l < LW; ++l) load_dz(m_a - OB0 + l - 1, win[l]);
+      int rs = 0;
+      for (int mm = 0; mm < nstep; ++mm) {
+        const int m = m_a + mm;
+#pragma unroll
+        for (int l = 0; l + 1 < LW; ++l)
+#pragma unroll
+          for (int j = 0; j < NDZ; ++j)
+#pragma unroll
+            for (int i = 0; i < V; ++i) win[l][j][i] = win[l + 1][j][i];
+        cp_wait_pending(kFbDepth - 1);                          // this step's group has landed (own copies only)
+        const int o = m - OB0 + LW - 1;
+#pragma unroll
+        for (int j = 0; j < NDZ; ++j) {
+          if (o < Fo && ((cmask >> j) & 1u)) {
+            float p[V], z[V];
+            ring(rs, j, p);
+            ring(rs, NDZ + j, z);
+            dz_of(p, z, win[LW - 1][j]);
+          } else {
+#pragma unroll
+            for (int i = 0; i < V; ++i) win[LW - 1][j][i] = 0.f;
+          }
+        }
+        float xr[S][Q][V];                                      // raw input (z1 or the block input) at the own columns
+#pragma unroll
+        for (int r = 0; r < S; ++r)
+#pragma unroll
+          for (int q = 0; q < Q; ++q) {
+            if (S * m + r < F && ((qmask >> q) & 1u)) ring(rs, 2 * NDZ + r * Q + q, xr[r][q]);
+            else {
+#pragma unroll
+              for (int i = 0; i < V; ++i) xr[r][q][i] = 0.f;
+            }
+          }
+        issue(mm + kFbDepth, rs);                               // the slot just read takes the step `depth` ahead
+        if (++rs == kFbDepth) rs = 0;
+        float isc[V], ish[V];
+        if (XF) {
+          VecF<V>::load(bnl + 4 * cst, isc);
+          VecF<V>::load(bnl + 5 * cst, ish);
+        }
+#pragma unroll
+        for (int r = 0; r < S; ++r) {
+          const int irow = S * m + r;
+          if (irow >= F) continue;
+          float xf[Q][V];
+#pragma unroll
+          for (int q = 0; q < Q; ++q) {
+            const bool ok = (qmask >> q) & 1u;
+#pragma unroll
+            for (int i = 0; i < V; ++i) xf[q][i] = XF ? (ok ? xact<ACT>(fmaf(xr[r][q][i], isc[i], ish[i])) : 0.f) : xr[r][q][i];
+          }
+          float acc[Q][V];
+#pragma unroll
+          for (int q = 0; q < Q; ++q)
+#pragma unroll
+            for (int i = 0; i < V; ++i) acc[q][i] = 0.f;
+#pragma unroll
+          for (int ky = 0; ky < K; ++ky) {
+            if (S == 2 && ((r + PAD - ky) & 1) != 0) continue;
+            const int sl = S == 1 ? 2 * PAD - ky : (r + PAD - ky) / 2 + PAD / 2;   // dz row (i + PAD - ky) / S
+#pragma unroll
+            for (int kx = 0; kx < K; ++kx) {
+              float w[V];
+              VecF<V>::load(wl + (ky * K + kx) * cst, w);
+#pragma unroll
+              for (int q = 0; q < Q; ++q) {
+                if (S == 2 && ((q + PAD - kx) & 1) != 0) continue;
+                const int j = S == 1 ? q + 2 * PAD - kx : (q + PAD - kx) / 2 + PAD / 2;   // dz column (t + PAD - kx) / S
+                fma_vec<V>(win[sl][j], w, acc[q]);
+                fma_vec<V>(win[sl][j], xf[q], wacc[ky * K + kx]);
+              }
+            }
+          }
+#pragma unroll
+          for (int q = 0; q < Q; ++q) {
+            if (!((qmask >> q) & 1u)) continue;
+            const size_t off = ((size_t)irow * Tn + q) * C;
+            if (resp != nullptr) {
+              float rv[V];
+              VecF<V>::load(resp + off, rv);
+#pragma unroll
+              for (int i = 0; i < V; ++i) acc[q][i] += rv[i];
+            }
+            VecF<V>::store(dinp + off, acc[q]);
+            if (red) {
+              float mu[V];
+              VecF<V>::load(bnl + 6 * cst, mu);
+#pragma unroll
+              for (int i = 0; i < V; ++i) {
+                const float gd = acc[q][i] * act_bwd(fmaf(xr[r][q][i], isc[i], ish[i]), ACT);
+                lsum[i] += gd;
+                lsq[i] = fmaf(gd, xr[r][q][i] - mu[i], lsq[i]);
+              }
+            }
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < KK; ++q)
+#pragma unroll
+      for (int i = 0; i < V; ++i) atomicAdd(&s_acc[q * cst + cvl * V + i], wacc[q][i]);
+    if (red) {
+#pragma unroll
+      for (int i = 0; i < V; ++i) { atomicAdd(&s_red[cvl * V + i], lsum[i]); atomicAdd(&s_red[cst + cvl * V + i], lsq[i]); }
+    }
+  }
+  __syncthreads();
+  for (int i = tid; i < KK * cc; i += kST) {
+    const int q = i / cc, c = i - q * cc;
+    atomicAdd(a.dw + (size_t)(cv0 * V + c) * KK + q, s_acc[q * cst + c]);
+  }
+  if (red) {
+    for (int c = tid; c < cc; c += kST) {
+      const int cg = cv0 * V + c;
+      atomicAdd(a.s1 + cg, (double)s_red[c]);
+      atomicAdd(a.s2 + cg, (double)s_red[cst + c] * (double)__ldg(a.zinvstd + cg));
+    }
+  }
+}
+
+template <int K, int S, int ACT, bool XF>
+int launch_fb_one(const FusedBwdArgs& a, dim3 grid, size_t smem, cudaStream_t st) {
+  static unsigned long long mask = 0;
+  if (int rc = eat_opt_in_smem(dw_bwd_fused_kernel<K, S, ACT, XF>, 64 * 1024, mask)) return rc;
+  dw_bwd_fused_kernel<K, S, ACT, XF><<<grid, kST, smem, st>>>(a);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+// a step reads LW dz rows, consecutive steps share LW - 1 of them: the plan of a stride-1 walk with an LW-row kernel over
+// the steps (din rows, or row pairs for stride 2) and Q-wide din strips
+template <int K, int S>
+SlidePlan plan_fb(int B, int F, int Tn, int C) {
+  using Sh = FbShape<K, S>;
+  const int rows = S == 1 ? F : (F + 1) / 2;
+  return plan_slide(B, rows, Tn, C / Sh::V, Sh::V, Sh::Q, 1, Sh::LW, Sh::MINB, false, kFbCvcMax);
+}
+
+template <int K, int S>
+int launch_fb(FusedBwdArgs a, int act, bool xf, cudaStream_t st) {
+  using Sh = FbShape<K, S>;
+  const SlidePlan pl = plan_fb<K, S>(a.B, a.F, a.Tn, a.C);
+  a.chunks = pl.chunks; a.cvc = pl.cvc; a.seg_rows = pl.seg_rows;
+  dim3 grid(pl.chunks * pl.groups, pl.gy);
+  const size_t smem = (size_t)(2 * K * K + 9) * a.cvc * Sh::V * sizeof(float) +
+                      (size_t)kFbDepth * Sh::NV * kST * Sh::V * sizeof(float);
+  if (act == EAT_ACT_RELU) return xf ? launch_fb_one<K, S, EAT_ACT_RELU, true>(a, grid, smem, st)
+                                     : launch_fb_one<K, S, EAT_ACT_RELU, false>(a, grid, smem, st);
+  return xf ? launch_fb_one<K, S, EAT_ACT_HSWISH, true>(a, grid, smem, st)
+            : launch_fb_one<K, S, EAT_ACT_HSWISH, false>(a, grid, smem, st);
+}
+
 }  // namespace
+
+extern "C" int eat_dw_conv_bwd_fused(const float* dp, const float* gate, const float* dpool, const float* z2,
+                                     const float* scale, const float* shift, const float* mean, const float* invstd, int act,
+                                     const float* c1, const float* c2, const float* wt, const float* in,
+                                     const float* in_scale, const float* in_shift, int in_act, const float* res, float* din,
+                                     float* dw, const float* zmean, const float* zinvstd, double* s1, double* s2, int dtype,
+                                     int B, int F, int T, int C, int k, int stride, cudaStream_t st) {
+  if (dtype != EAT_F32) { eat_set_error("dw_conv_bwd_fused: fp32 storage only"); return EAT_ERR_UNSUPPORTED; }
+  if ((k != 3 && k != 5) || (stride != 1 && stride != 2)) {
+    eat_set_error("dw_conv_bwd_fused: k in {3,5}, stride in {1,2} only");
+    return EAT_ERR_UNSUPPORTED;
+  }
+  const int V = k == 3 ? 4 : 2;
+  if (C <= 0 || C % V != 0) {
+    eat_set_error(k == 3 ? "dw_conv_bwd_fused: 3x3 needs channels in multiples of 4" : "dw_conv_bwd_fused: 5x5 needs channels in multiples of 2");
+    return EAT_ERR_UNSUPPORTED;
+  }
+  if (act != EAT_ACT_RELU && act != EAT_ACT_HSWISH) { eat_set_error("dw_conv_bwd_fused: activation must be relu or hardswish"); return EAT_ERR_UNSUPPORTED; }
+  if (in_scale != nullptr && (in_shift == nullptr || in_act != act)) {
+    eat_set_error("dw_conv_bwd_fused: the input transform needs in_shift and the block's activation (in_act == act)");
+    return EAT_ERR_UNSUPPORTED;
+  }
+  if (dp == nullptr || z2 == nullptr || scale == nullptr || shift == nullptr || mean == nullptr || invstd == nullptr ||
+      c1 == nullptr || c2 == nullptr || wt == nullptr || in == nullptr || din == nullptr || dw == nullptr) {
+    eat_set_error("dw_conv_bwd_fused: dp, z2, the BN2 tables, c1/c2, wt, in, din and dw are required");
+    return EAT_ERR_ARG;
+  }
+  if (s1 != nullptr && (s2 == nullptr || zmean == nullptr || zinvstd == nullptr || in_scale == nullptr)) {
+    eat_set_error("dw_conv_bwd_fused: the BN1 reduce needs s2, zmean, zinvstd and the input transform");
+    return EAT_ERR_ARG;
+  }
+  if (B < 0 || F < 0 || T < 0) { eat_set_error("dw_conv_bwd_fused: negative shape"); return EAT_ERR_ARG; }
+  if (B == 0 || F == 0 || T == 0) return EAT_OK;
+  const int pad = (k - 1) / 2;
+  FusedBwdArgs a;
+  a.dp = dp; a.gate = gate; a.dpool = dpool; a.z2 = z2;
+  a.scale = scale; a.shift = shift; a.mean = mean; a.invstd = invstd; a.c1 = c1; a.c2 = c2;
+  a.wt = wt; a.in = in; a.in_scale = in_scale; a.in_shift = in_shift; a.res = res; a.din = din; a.dw = dw;
+  a.zmean = zmean; a.zinvstd = zinvstd; a.s1 = s1; a.s2 = s2;
+  a.B = B; a.F = F; a.Tn = T; a.C = C;
+  a.Fo = (F + 2 * pad - k) / stride + 1;
+  a.To = (T + 2 * pad - k) / stride + 1;
+  const bool xf = in_scale != nullptr;
+  if (k == 3) return stride == 1 ? launch_fb<3, 1>(a, act, xf, st) : launch_fb<3, 2>(a, act, xf, st);
+  return stride == 1 ? launch_fb<5, 1>(a, act, xf, st) : launch_fb<5, 2>(a, act, xf, st);
+}
 
 int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
                     InXform xf, const float* scale, const float* shift, int act, const void* res, int flip, float* pool,
@@ -1143,10 +1568,21 @@ int dw_dgrad2_slide_launch(const void* dz, const float* wt, long long wt_bstride
 }
 
 extern "C" int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int k, int stride, int per_sample, int* plan) {
-  const int V0 = dtype == EAT_BF16 ? 8 : 4;
+  const int V0 = kind == 3 ? (k == 5 ? 2 : 4) : (dtype == EAT_BF16 ? 8 : 4);
   if (plan == nullptr || B < 1 || F < 1 || T < 1 || C % V0 != 0 || (k != 3 && k != 5) || (stride != 1 && stride != 2)) {
     eat_set_error("dw_plan: invalid arguments");
     return EAT_ERR_ARG;
+  }
+  if (kind == 3) {                                   // dw_bwd_fused_kernel: steps (din rows / row pairs), Q din columns
+    if (dtype != EAT_F32) { eat_set_error("dw_plan: the fused depthwise backward is fp32 only"); return EAT_ERR_UNSUPPORTED; }
+    SlidePlan pl;
+    int Q;
+    if (k == 3 && stride == 1) { pl = plan_fb<3, 1>(B, F, T, C); Q = FbShape<3, 1>::Q; }
+    else if (k == 3) { pl = plan_fb<3, 2>(B, F, T, C); Q = FbShape<3, 2>::Q; }
+    else if (stride == 1) { pl = plan_fb<5, 1>(B, F, T, C); Q = FbShape<5, 1>::Q; }
+    else { pl = plan_fb<5, 2>(B, F, T, C); Q = FbShape<5, 2>::Q; }
+    plan[0] = pl.chunks; plan[1] = pl.cvc; plan[2] = pl.seg_rows; plan[3] = pl.groups; plan[4] = pl.gy; plan[5] = Q;
+    return EAT_OK;
   }
   const bool f32 = dtype != EAT_BF16;
   const int pad = (k - 1) / 2;
@@ -1167,7 +1603,7 @@ extern "C" int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int 
     P = 4; minb = k == 3 ? 4 : 3;
     rows = (F + 1) / 2; cols = T; S = 1; Kp = (k + 1) / 2;
   } else {
-    eat_set_error("dw_plan: kind must be 0, 1 or 2");
+    eat_set_error("dw_plan: kind must be 0, 1, 2 or 3");
     return EAT_ERR_ARG;
   }
   const SlidePlan pl = plan_slide(B, rows, cols, C / V, V, P, S, Kp, minb, per_sample != 0);

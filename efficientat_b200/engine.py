@@ -48,6 +48,14 @@ SE_FUSED_DEFAULT = "1"
 DGRAD_BNRED_DEFAULT = "0"
 
 
+# fp32 storage: the depthwise stage's backward below its BatchNorm (BN2 apply, weight and data gradient, expand-BatchNorm
+# reduce) as one kernel, eat_dw_conv_bwd_fused; EAT_DW_BWD_FUSED=0 restores the four passes.  Routed (k, stride): at the
+# mn10 B=256 shapes the fused kernel is 1.5-2.2x faster than the four passes for 3x3 and 5x5 stride 2, but 5x5 stride 1
+# (blocks 5-6: 1.1x, blocks 14-15 at 4x32 pixels: 0.64x) loses in total, so those layers keep the passes
+DW_BWD_FUSED_DEFAULT = "1"
+DW_BWD_FUSED_SHAPES = ((3, 1), (3, 2), (5, 2))
+
+
 class _ZeroPool:
     """fp64 accumulators for BatchNorm statistics, carved from chunks that are zeroed with ONE fill each
     (a training step needs ~100 small zeroed buffers; one launch per buffer showed up as 250 tiny kernels)."""
@@ -110,6 +118,9 @@ class MNEngine:
         # stride-2 blocks: the BatchNorm-backward reduce of the expand stage inside the depthwise data-gradient kernel that
         # produces its upstream gradient (eat_dw_conv_dgrad_bnred), fp32 storage
         self.dgrad_bnred = os.environ.get("EAT_DGRAD_BNRED", DGRAD_BNRED_DEFAULT) == "1"
+        # fp32 storage: BN2-backward apply, depthwise weight and data gradient and the expand BatchNorm's reduce in one walk
+        # (eat_dw_conv_bwd_fused); takes precedence over dgrad_bnred
+        self.dw_bwd_fused = os.environ.get("EAT_DW_BWD_FUSED", DW_BWD_FUSED_DEFAULT) == "1"
         self._fork = None
         self._se_scale = {}
         self._zero_pool = _ZeroPool()
@@ -475,12 +486,10 @@ class MNEngine:
         else:
             lib().gemm_simt_wgrad(*args)
 
-    def _bn_bwd(self, gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code=None, sums=None):
-        """two-pass BatchNorm(+activation) backward -> dz (same dtype/shape as z).  `sums`: the (s1, s2) accumulators when
-        the reduce pass already happened elsewhere (SE blocks: eat_se_bn_bwd_reduce + eat_se_bn_bwd_combine)."""
+    def _bn_bwd_coef(self, gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code, sums):
+        """BatchNorm-backward reduce (unless `sums` holds it already) + finalize -> the apply pass's (c1, c2) [2, C]"""
         L = lib()
         st = _stream()
-        code = self.dcode if code is None else code
         if sums is None:
             s = self._zero_pool.take(2, C, dev)
             L.bn_bwd_reduce(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
@@ -490,6 +499,15 @@ class MNEngine:
         coef = torch.empty(2, C, device=dev, dtype=torch.float32)
         L.bn_bwd_finalize(s[0].data_ptr(), s[1].data_ptr(), float(B * P), _ptr(dgamma), _ptr(dbeta),
                           coef[0].data_ptr(), coef[1].data_ptr(), C, st)
+        return coef
+
+    def _bn_bwd(self, gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code=None, sums=None):
+        """two-pass BatchNorm(+activation) backward -> dz (same dtype/shape as z).  `sums`: the (s1, s2) accumulators when
+        the reduce pass already happened elsewhere (SE blocks: eat_se_bn_bwd_reduce + eat_se_bn_bwd_combine)."""
+        L = lib()
+        st = _stream()
+        code = self.dcode if code is None else code
+        coef = self._bn_bwd_coef(gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code, sums)
         dz = torch.empty_like(z)
         L.bn_bwd_apply(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
                        sv[0].data_ptr(), sv[1].data_ptr(), act, coef[0].data_ptr(), coef[1].data_ptr(), dz.data_ptr(),
@@ -546,11 +564,28 @@ class MNEngine:
             sums2 = self._zero_pool.take(2, blk.cexp, dev)
             L.se_bn_bwd_combine(part.data_ptr(), parts, gate.data_ptr(), dpool.data_ptr(), R["sv2"][1].data_ptr(), B,
                                 blk.cexp, sums2[0].data_ptr(), sums2[1].data_ptr(), st)
-        dz2 = self._bn_bwd(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
-                           G[blk.dw[1].weight], G[blk.dw[1].bias], dev, sums=sums2)
         has_exp = blk.expand is not None
         dw_in = R["z1"] if has_exp else R["inp"]
         sc1 = R["sc1"] if has_exp else None
+        if (self.dw_bwd_fused and dc == 0 and (blk.k, blk.stride) in DW_BWD_FUSED_SHAPES
+                and blk.cexp % (4 if blk.k == 3 else 2) == 0):      # the kernel's channel vector: 4 (3x3) or 2 (5x5)
+            # dz2 is computed on load and never stored; one walk yields the depthwise input gradient, the depthwise
+            # weight gradient and the expand BatchNorm's backward sums
+            coef = self._bn_bwd_coef(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
+                                     G[blk.dw[1].weight], G[blk.dw[1].bias], dev, dc, sums2)
+            da1 = torch.empty_like(dw_in)
+            sums1 = self._zero_pool.take(2, blk.cexp, dev) if has_exp else None
+            L.dw_conv_bwd_fused(dp.data_ptr(), _ptr(gate), _ptr(dpool), R["z2"].data_ptr(), R["sc2"][0].data_ptr(),
+                                R["sc2"][1].data_ptr(), R["sv2"][0].data_ptr(), R["sv2"][1].data_ptr(), blk.act,
+                                coef[0].data_ptr(), coef[1].data_ptr(), R["wt"].data_ptr(), dw_in.data_ptr(),
+                                _ptr(sc1[0]) if has_exp else 0, _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0,
+                                _ptr(dy) if (blk.res and not has_exp) else 0, da1.data_ptr(),
+                                G[blk.dw[0].weight].data_ptr(), _ptr(R["sv1"][0]) if has_exp else 0,
+                                _ptr(R["sv1"][1]) if has_exp else 0, _ptr(sums1[0]) if has_exp else 0,
+                                _ptr(sums1[1]) if has_exp else 0, dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, st)
+            return self._expand_bwd(blk, R, dy, G, B, da1, sums1)
+        dz2 = self._bn_bwd(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
+                           G[blk.dw[1].weight], G[blk.dw[1].bias], dev, sums=sums2)
         fork.run(lambda: L.dw_conv_wgrad(dz2.data_ptr(), dw_in.data_ptr(), _ptr(sc1[0]) if has_exp else 0,
                                          _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0,
                                          G[blk.dw[0].weight].data_ptr(), 0, dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
@@ -568,17 +603,23 @@ class MNEngine:
             # without an expand stage the depthwise input IS the block input: fold the residual gradient in
             L.dw_conv_dgrad(dz2.data_ptr(), R["wt"].data_ptr(), 0, _ptr(dy) if (blk.res and not has_exp) else 0,
                             da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, st)
-        if has_exp:
-            dz1 = self._bn_bwd(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
-                               G[blk.expand[1].weight], G[blk.expand[1].bias], dev, sums=sums1)
-            fork.run(lambda: self._wgrad(dz1, R["inp"], G[blk.expand[0].weight], None, B * Pi, blk.cexp, blk.cin), dz1)
-            dinp = torch.empty_like(R["inp"])
-            self._gemm(dz1, blk.expand[0].weight, dinp, B * Pi, blk.cin, blk.cexp, w_trans=True,
-                       res=dy if blk.res else None)
-            dy = dinp
-        else:
-            dy = da1
-        return dy
+        return self._expand_bwd(blk, R, dy, G, B, da1, sums1)
+
+    def _expand_bwd(self, blk, R, dy, G, B, da1, sums1):
+        """expand stage (BN1 + 1x1 conv) from the depthwise input gradient da1; returns the gradient w.r.t. the block input.
+        sums1: BN1's backward sums when the depthwise backward already took them (else None: a reduce pass)."""
+        if blk.expand is None:
+            return da1
+        dev = da1.device
+        Pi = R["Fi"] * R["Ti"]
+        fork = self._fork if self._fork is not None else _Fork(dev, False)
+        dz1 = self._bn_bwd(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
+                           G[blk.expand[1].weight], G[blk.expand[1].bias], dev, sums=sums1)
+        fork.run(lambda: self._wgrad(dz1, R["inp"], G[blk.expand[0].weight], None, B * Pi, blk.cexp, blk.cin), dz1)
+        dinp = torch.empty_like(R["inp"])
+        self._gemm(dz1, blk.expand[0].weight, dinp, B * Pi, blk.cin, blk.cexp, w_trans=True,
+                   res=dy if blk.res else None)
+        return dinp
 
     def _backward(self, S, dlogits, on_ready=None):
         """-> dict {parameter: fp32 gradient view into one flat arena} (arena returned under key None).

@@ -47,9 +47,11 @@ const char* eat_last_error(void);
 int eat_abi_version(void);
 
 /* Host-only (no GPU work): the launch plan of the sliding-window depthwise kernels (csrc/dw_slide.cu) for a layer.
- * kind: 0 forward, 1 weight gradient, 2 stride-2 data gradient.  per_sample != 0: blockIdx.y must be the sample
- * (squeeze-excitation pooling, DynamicConv per-sample weights).  plan[6] = {channel chunks, channel vectors per chunk,
- * output rows (row pairs for kind 2) per segment, CTA groups per chunk, gridDim.y, strip width}.  Exposed so the
+ * kind: 0 forward, 1 weight gradient, 2 stride-2 data gradient, 3 fused backward (eat_dw_conv_bwd_fused, fp32; its
+ * channel vectors are 4 channels for 3x3 and 2 for 5x5).  per_sample != 0: blockIdx.y must be the sample
+ * (squeeze-excitation pooling, DynamicConv per-sample weights; ignored by kind 3).  plan[6] = {channel chunks, channel
+ * vectors per chunk, output rows (row pairs for kind 2; din rows, or row pairs for stride 2, for kind 3) per segment,
+ * CTA groups per chunk, gridDim.y, strip width}.  Exposed so the
  * host logic is testable without a device (tests/test_cabi.py). */
 int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int k, int stride, int per_sample, int* plan);
 int eat_device_check(int device);
@@ -276,6 +278,20 @@ int eat_dw_conv_dgrad_bnred(const void* dz, const float* wt, const void* res, vo
 int eat_dw_conv_wgrad(const void* dz, const void* in, const float* in_scale, const float* in_shift, int in_act,
                       float* dw, long long dw_bstride, int dtype, int B, int F, int T, int C, int k, int stride,
                       cudaStream_t stream);   /* wt_bstride / dw_bstride: floats between per-sample tables (0: shared) */
+/* The depthwise stage's backward in one pass, from the upstream gradient dp [B,Fo,To,C] of its BatchNorm + activation
+ * (BN2, raw output z2 [B,Fo,To,C]) down to the input: dz = eat_bn_bwd_apply(dp, gate, dpool, z2, scale ... c2) is
+ * computed on load and never stored; din [B,F,T,C] = data gradient of dz (+ res); dw [C,1,k,k] += weight gradient of
+ * dz against xf(in) = act(in*in_scale+in_shift) (identity when in_scale is NULL; in_act must equal act); and, unless s1 is
+ * NULL, the BatchNorm-backward reduce of the expand stage behind din (s1[c] += sum g, s2[c] += zinvstd[c] *
+ * sum g*(in-zmean[c]), g = din * act'(in*in_scale+in_shift)), as eat_dw_conv_dgrad_bnred.  c1/c2 come from
+ * eat_bn_bwd_finalize of BN2's sums.  fp32 storage, k in {3,5}, stride in {1,2}, act relu or hardswish, C a multiple of
+ * 4 (3x3) or 2 (5x5); anything else returns EAT_ERR_UNSUPPORTED before any launch. */
+int eat_dw_conv_bwd_fused(const float* dp, const float* gate, const float* dpool, const float* z2, const float* scale,
+                          const float* shift, const float* mean, const float* invstd, int act, const float* c1,
+                          const float* c2, const float* wt, const float* in, const float* in_scale, const float* in_shift,
+                          int in_act, const float* res, float* din, float* dw, const float* zmean, const float* zinvstd,
+                          double* s1, double* s2, int dtype, int B, int F, int T, int C, int k, int stride,
+                          cudaStream_t stream);
 /* Stem weight gradient (the spectrogram itself needs no gradient). */
 int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, int F, int T, int C, int stride,
                    cudaStream_t stream);
