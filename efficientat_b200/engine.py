@@ -56,6 +56,12 @@ DW_BWD_FUSED_DEFAULT = "1"
 DW_BWD_FUSED_SHAPES = ((3, 1), (3, 2), (5, 2))
 
 
+# fp32 storage: the expand stage's backward below its BatchNorm (BN1 apply, weight and data gradient of the 1x1 conv) as one
+# kernel, eat_pw_conv_bwd_fused, for the shapes its planner takes (cin <= 32, cexp <= 128: mn10 blocks 2-4, where it is
+# 2.2-2.4x faster than the three passes at B=256); EAT_EXPAND_BWD_FUSED=0 restores the three passes
+EXPAND_BWD_FUSED_DEFAULT = "1"
+
+
 class _ZeroPool:
     """fp64 accumulators for BatchNorm statistics, carved from chunks that are zeroed with ONE fill each
     (a training step needs ~100 small zeroed buffers; one launch per buffer showed up as 250 tiny kernels)."""
@@ -121,6 +127,9 @@ class MNEngine:
         # fp32 storage: BN2-backward apply, depthwise weight and data gradient and the expand BatchNorm's reduce in one walk
         # (eat_dw_conv_bwd_fused); takes precedence over dgrad_bnred
         self.dw_bwd_fused = os.environ.get("EAT_DW_BWD_FUSED", DW_BWD_FUSED_DEFAULT) == "1"
+        # fp32 storage: BN1-backward apply and both expand GEMMs in one pass (eat_pw_conv_bwd_fused)
+        self.expand_bwd_fused = os.environ.get("EAT_EXPAND_BWD_FUSED", EXPAND_BWD_FUSED_DEFAULT) == "1"
+        self._pw_bwd_ok = {}
         self._fork = None
         self._se_scale = {}
         self._zero_pool = _ZeroPool()
@@ -612,6 +621,18 @@ class MNEngine:
             return da1
         dev = da1.device
         Pi = R["Fi"] * R["Ti"]
+        if self.expand_bwd_fused and self.dcode == 0 and self._pw_bwd_fused_takes(B * Pi, blk.cexp, blk.cin):
+            # dz1 is computed on load and never stored; one pass yields the block input's gradient and the expand weight's
+            coef = self._bn_bwd_coef(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
+                                     G[blk.expand[1].weight], G[blk.expand[1].bias], dev, 0, sums1)
+            dinp = torch.empty_like(R["inp"])
+            sc1, sv1 = R["sc1"], R["sv1"]
+            lib().pw_conv_bwd_fused(da1.data_ptr(), R["z1"].data_ptr(), sc1[0].data_ptr(), sc1[1].data_ptr(),
+                                    sv1[0].data_ptr(), sv1[1].data_ptr(), blk.act, coef[0].data_ptr(), coef[1].data_ptr(),
+                                    R["inp"].data_ptr(), blk.expand[0].weight.data_ptr(), _ptr(dy) if blk.res else 0,
+                                    dinp.data_ptr(), G[blk.expand[0].weight].data_ptr(), 0, B * Pi, blk.cexp, blk.cin,
+                                    _stream())
+            return dinp
         fork = self._fork if self._fork is not None else _Fork(dev, False)
         dz1 = self._bn_bwd(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
                            G[blk.expand[1].weight], G[blk.expand[1].bias], dev, sums=sums1)
@@ -620,6 +641,20 @@ class MNEngine:
         self._gemm(dz1, blk.expand[0].weight, dinp, B * Pi, blk.cin, blk.cexp, w_trans=True,
                    res=dy if blk.res else None)
         return dinp
+
+    def _pw_bwd_fused_takes(self, M, cexp, cin):
+        """whether eat_pw_conv_bwd_fused's planner accepts the expand stage (host-only, asked once per shape)"""
+        key = (M, cexp, cin)
+        if key not in self._pw_bwd_ok:
+            import ctypes
+            from ._lib import EatError
+            plan = (ctypes.c_int * 4)()
+            try:
+                lib().pw_bwd_plan(M, cexp, cin, ctypes.addressof(plan))
+                self._pw_bwd_ok[key] = True
+            except EatError:
+                self._pw_bwd_ok[key] = False
+        return self._pw_bwd_ok[key]
 
     def _backward(self, S, dlogits, on_ready=None):
         """-> dict {parameter: fp32 gradient view into one flat arena} (arena returned under key None).

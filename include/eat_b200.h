@@ -292,6 +292,21 @@ int eat_dw_conv_bwd_fused(const float* dp, const float* gate, const float* dpool
                           int in_act, const float* res, float* din, float* dw, const float* zmean, const float* zinvstd,
                           double* s1, double* s2, int dtype, int B, int F, int T, int C, int k, int stride,
                           cudaStream_t stream);
+/* The expand stage's backward (1x1 conv + BatchNorm + activation, models/mn/block_types.py:140-147) in one pass, from
+ * the gradient da [M, cexp] at its output and its raw output z [M, cexp]: dz = eat_bn_bwd_apply(da, NULL, NULL, z, scale
+ * ... c2) is computed on load and never stored; dX [M, cin] = dz . W (+ res [M, cin]) with W the expand weight
+ * [cexp, cin]; dW [cexp, cin] += dz^T . X (zeroed by the caller, atomically accumulated).  c1/c2 come from
+ * eat_bn_bwd_finalize of the BatchNorm's backward sums.  bf16x3 tensor-core products (~2^-16 relative, as eat_pw_tma_fwd
+ * and eat_pw_tma_wgrad).  fp32 storage, act relu or hardswish, cin <= 32 and cexp <= 128, both multiples of 4;
+ * anything else returns EAT_ERR_UNSUPPORTED / EAT_ERR_ARG before any launch.  M == 0 is a no-op. */
+int eat_pw_conv_bwd_fused(const float* da, const float* z, const float* scale, const float* shift, const float* mean,
+                          const float* invstd, int act, const float* c1, const float* c2, const float* X, const float* W,
+                          const float* res, float* dX, float* dW, int dtype, long long M, int cexp, int cin,
+                          cudaStream_t stream);
+/* Host-only (no GPU work): whether eat_pw_conv_bwd_fused takes a shape (EAT_OK) or not (EAT_ERR_UNSUPPORTED /
+ * EAT_ERR_ARG), and its launch on a 132-SM H100: plan[4] = {CTAs (one per SM at most, each a contiguous range of
+ * 128-row tiles), rows per CTA at most, pipeline stages, dynamic shared-memory bytes}. */
+int eat_pw_bwd_plan(long long M, int cexp, int cin, int* plan);
 /* Stem weight gradient (the spectrogram itself needs no gradient). */
 int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, int F, int T, int C, int stride,
                    cudaStream_t stream);
