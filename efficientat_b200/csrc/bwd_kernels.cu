@@ -736,12 +736,16 @@ __global__ void __launch_bounds__(kThreads) stem_wgrad_kernel(const T* __restric
 
 // Row-oriented stem weight gradient (fp32 dz, C <= 64): same walk as stem_row_kernel; the U = 4 gradient vectors and
 // the 36 input values of a trip are requested before the first use (the pixel-at-a-time kernel above has ONE 16-byte
-// load in flight per thread).
-template <int S>
-__global__ void __launch_bounds__(kThreads) stem_wgrad_row_kernel(const float* __restrict__ dz, const float* __restrict__ x,
+// load in flight per thread).  APPLY: `dz` is the gradient dy at the BatchNorm + activation's output and dz is computed
+// on load from (dy, z) with the folded constants of eat_bn_bwd_apply (as bn_bwd_apply2_kernel), so the stem's
+// BatchNorm-backward apply pass and its dz tensor are not needed.
+template <int S, int APPLY>
+__global__ void __launch_bounds__(kThreads, APPLY ? 2 : 1) stem_wgrad_row_kernel(const float* __restrict__ dz, const float* __restrict__ x,
                                                                   float* __restrict__ dw, int B, int F, int Tn, int Fo,
-                                                                  int To, int C) {
-  constexpr int V = 4, U = 4;
+                                                                  int To, int C, const float* __restrict__ z, BnCtx bn,
+                                                                  int act, const float* __restrict__ c1,
+                                                                  const float* __restrict__ c2) {
+  constexpr int V = 4, U = APPLY ? 2 : 4;        // 64 bytes of dz (dy and z) loads in flight either way
   __shared__ float s_acc[9 * 64];
   for (int i = threadIdx.x; i < 9 * C; i += kThreads) s_acc[i] = 0.f;
   __syncthreads();
@@ -754,19 +758,31 @@ __global__ void __launch_bounds__(kThreads) stem_wgrad_row_kernel(const float* _
     for (int q = 0; q < 9; ++q)
 #pragma unroll
       for (int k = 0; k < V; ++k) acc[q][k] = 0.f;
+    float sc[V], sh[V], al[V], be[V];              // dz = sc * (dy * act'(z * sc + sh)) + al * z + be
+    if (APPLY) {
+#pragma unroll
+      for (int k = 0; k < V; ++k) {
+        const int c = cvi * V + k;
+        sc[k] = bn.scale[c]; sh[k] = bn.shift[c];
+        al[k] = -sc[k] * c2[c] * bn.invstd[c];
+        be[k] = -sc[k] * c1[c] - al[k] * bn.mean[c];
+      }
+    }
     const int rows = B * Fo;
     for (int row = blockIdx.x; row < rows; row += gridDim.x) {
       const int b = row / Fo, fo = row - b * Fo;
       const float* xb = x + (size_t)b * F * Tn;
       const float* grow = dz + (size_t)row * To * C + cvi * V;
+      const float* zrow = APPLY ? z + (size_t)row * To * C + cvi * V : nullptr;
       const int f0 = fo * S - 1;
       for (int to0 = slot; to0 < To; to0 += U * ppb) {
-        float4 g[U];
+        float4 g[U], zz[U];
         float xv[U][9];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int to = to0 + u * ppb, t0 = to * S - 1;
           g[u] = to < To ? *reinterpret_cast<const float4*>(grow + (size_t)to * C) : make_float4(0.f, 0.f, 0.f, 0.f);
+          if (APPLY) zz[u] = to < To ? *reinterpret_cast<const float4*>(zrow + (size_t)to * C) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
           for (int ky = 0; ky < 3; ++ky) {
             const int f = f0 + ky;
@@ -779,7 +795,16 @@ __global__ void __launch_bounds__(kThreads) stem_wgrad_row_kernel(const float* _
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-          const float gv[V] = {g[u].x, g[u].y, g[u].z, g[u].w};
+          float gv[V] = {g[u].x, g[u].y, g[u].z, g[u].w};
+          if (APPLY) {
+            const float zv[V] = {zz[u].x, zz[u].y, zz[u].z, zz[u].w};
+            const bool live = to0 + u * ppb < To;      // past the row's end dz is 0, not beta
+#pragma unroll
+            for (int k = 0; k < V; ++k) {
+              const float gg = gv[k] * act_bwd(fmaf(zv[k], sc[k], sh[k]), act);
+              gv[k] = live ? fmaf(sc[k], gg, fmaf(al[k], zv[k], be[k])) : 0.f;
+            }
+          }
 #pragma unroll
           for (int q = 0; q < 9; ++q)
 #pragma unroll
@@ -1048,19 +1073,34 @@ int eat_dw_conv_wgrad(const void* dz, const void* in, const float* in_scale, con
 }
 
 int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, int F, int T, int C, int stride,
-                   cudaStream_t st) {
+                   const float* z, const float* scale, const float* shift, const float* mean, const float* invstd, int act,
+                   const float* c1, const float* c2, cudaStream_t st) {
   const int Fo = (F + 2 - 3) / stride + 1, To = (T + 2 - 3) / stride + 1;
   const int V = dtype == EAT_BF16 ? 8 : 4;
   if (C % V != 0 || C / V > kThreads) { eat_set_error("stem wgrad: unsupported channel count"); return EAT_ERR_ARG; }
+  const bool rowk = dtype == EAT_F32 && C <= 64 && (stride == 1 || stride == 2);
+  if (z != nullptr) {
+    if (!rowk) {
+      eat_set_error("stem wgrad: the BatchNorm apply on load needs fp32 storage, C <= 64 and stride 1 or 2");
+      return EAT_ERR_UNSUPPORTED;
+    }
+    if (scale == nullptr || shift == nullptr || mean == nullptr || invstd == nullptr || c1 == nullptr || c2 == nullptr) {
+      eat_set_error("stem wgrad: the BatchNorm apply on load needs scale, shift, mean, invstd, c1 and c2");
+      return EAT_ERR_ARG;
+    }
+  }
   const long long npix = (long long)B * Fo * To;
   if (npix == 0) return EAT_OK;
   if (npix >= (1ll << 31)) { eat_set_error("stem wgrad: B*Fo*To must be below 2^31"); return EAT_ERR_ARG; }
   const int ppb = kThreads / (C / V);
-  if (dtype == EAT_F32 && C <= 64 && (stride == 1 || stride == 2)) {
+  if (rowk) {
     const int rows = B * Fo;
     const int grid_r = rows < kNumSMs * 6 ? rows : kNumSMs * 6;
-    if (stride == 2) stem_wgrad_row_kernel<2><<<grid_r, kThreads, 0, st>>>((const float*)dz, x, dw, B, F, T, Fo, To, C);
-    else stem_wgrad_row_kernel<1><<<grid_r, kThreads, 0, st>>>((const float*)dz, x, dw, B, F, T, Fo, To, C);
+    const BnCtx bn{scale, shift, mean, invstd};
+#define EAT_STEM_WG(S_, A_) stem_wgrad_row_kernel<S_, A_><<<grid_r, kThreads, 0, st>>>((const float*)dz, x, dw, B, F, T, Fo, To, C, z, bn, act, c1, c2)
+    if (stride == 2) { if (z != nullptr) EAT_STEM_WG(2, 1); else EAT_STEM_WG(2, 0); }
+    else { if (z != nullptr) EAT_STEM_WG(1, 1); else EAT_STEM_WG(1, 0); }
+#undef EAT_STEM_WG
     EAT_CHECK_LAUNCH();
     return EAT_OK;
   }

@@ -62,6 +62,17 @@ DW_BWD_FUSED_SHAPES = ((3, 1), (3, 2), (5, 2))
 EXPAND_BWD_FUSED_DEFAULT = "1"
 
 
+# fp32 storage: the project stage's backward below BN3 (BN3 apply, weight and data gradient of the 1x1 conv, BN2's reduce)
+# as one kernel, eat_pw_proj_bwd_fused, for blocks without SE whose shapes its planner takes (cout <= 32, cexp <= 128:
+# mn10 blocks 1-3); EAT_PROJ_BWD_FUSED=0 restores the separate passes
+PROJ_BWD_FUSED_DEFAULT = "1"
+
+
+# fp32 storage: the stem BatchNorm's backward apply on load in the stem weight gradient (eat_stem_wgrad with z), its only
+# consumer, instead of a pass that writes dz0; EAT_STEM_BWD_FUSED=0 restores the apply pass
+STEM_BWD_FUSED_DEFAULT = "1"
+
+
 class _ZeroPool:
     """fp64 accumulators for BatchNorm statistics, carved from chunks that are zeroed with ONE fill each
     (a training step needs ~100 small zeroed buffers; one launch per buffer showed up as 250 tiny kernels)."""
@@ -129,6 +140,11 @@ class MNEngine:
         self.dw_bwd_fused = os.environ.get("EAT_DW_BWD_FUSED", DW_BWD_FUSED_DEFAULT) == "1"
         # fp32 storage: BN1-backward apply and both expand GEMMs in one pass (eat_pw_conv_bwd_fused)
         self.expand_bwd_fused = os.environ.get("EAT_EXPAND_BWD_FUSED", EXPAND_BWD_FUSED_DEFAULT) == "1"
+        # fp32 storage, blocks without SE: BN3-backward apply, both project GEMMs and BN2's backward reduce in one pass
+        # (eat_pw_proj_bwd_fused)
+        self.proj_bwd_fused = os.environ.get("EAT_PROJ_BWD_FUSED", PROJ_BWD_FUSED_DEFAULT) == "1"
+        # fp32 storage: the stem BatchNorm's backward apply inside the stem weight gradient (eat_stem_wgrad with z)
+        self.stem_bwd_fused = os.environ.get("EAT_STEM_BWD_FUSED", STEM_BWD_FUSED_DEFAULT) == "1"
         self._pw_bwd_ok = {}
         self._fork = None
         self._se_scale = {}
@@ -536,13 +552,27 @@ class MNEngine:
         Pi, Po = Fi * Ti, Fo * To
         gate = R.get("gate")
         # project: BN3 (no activation)
-        dz3 = self._bn_bwd(dy, None, None, R["z3"], R["sc3"], R["sv3"], 0, B, Po, blk.cout,
-                           G[blk.proj[1].weight], G[blk.proj[1].bias], dev)
         fork = self._fork if self._fork is not None else _Fork(dev, False)
-        fork.run(lambda: self._wgrad(dz3, R["z2"], G[blk.proj[0].weight], None, B * Po, blk.cout, blk.cexp, in_sc=R["sc2"],
-                                     in_act=blk.act, gate=gate, rows_per_sample=Po), dz3)
         dp = torch.empty_like(R["z2"])
-        self._gemm(dz3, blk.proj[0].weight, dp, B * Po, blk.cexp, blk.cout, w_trans=True)
+        sums2 = None                                    # BN2's backward sums, when a kernel above the depthwise took them
+        if (self.proj_bwd_fused and dc == 0 and blk.se is None
+                and self._plan_takes("pw_proj_bwd_plan", B * Po, blk.cexp, blk.cout)):
+            # dz3 is computed on load and never stored; one pass yields dp, the project weight's gradient and BN2's sums
+            coef = self._bn_bwd_coef(dy, None, None, R["z3"], R["sc3"], R["sv3"], 0, B, Po, blk.cout,
+                                     G[blk.proj[1].weight], G[blk.proj[1].bias], dev, 0, None)
+            sums2 = self._zero_pool.take(2, blk.cexp, dev)
+            sc3, sv3, sc2, sv2 = R["sc3"], R["sv3"], R["sc2"], R["sv2"]
+            L.pw_proj_bwd_fused(dy.data_ptr(), R["z3"].data_ptr(), sc3[0].data_ptr(), sc3[1].data_ptr(), sv3[0].data_ptr(),
+                                sv3[1].data_ptr(), coef[0].data_ptr(), coef[1].data_ptr(), R["z2"].data_ptr(),
+                                sc2[0].data_ptr(), sc2[1].data_ptr(), sv2[0].data_ptr(), sv2[1].data_ptr(), blk.act,
+                                blk.proj[0].weight.data_ptr(), dp.data_ptr(), G[blk.proj[0].weight].data_ptr(),
+                                sums2[0].data_ptr(), sums2[1].data_ptr(), 0, B * Po, blk.cexp, blk.cout, st)
+        else:
+            dz3 = self._bn_bwd(dy, None, None, R["z3"], R["sc3"], R["sv3"], 0, B, Po, blk.cout,
+                               G[blk.proj[1].weight], G[blk.proj[1].bias], dev)
+            fork.run(lambda: self._wgrad(dz3, R["z2"], G[blk.proj[0].weight], None, B * Po, blk.cout, blk.cexp,
+                                         in_sc=R["sc2"], in_act=blk.act, gate=gate, rows_per_sample=Po), dz3)
+            self._gemm(dz3, blk.proj[0].weight, dp, B * Po, blk.cexp, blk.cout, w_trans=True)
         dpool = None
         if blk.se is not None:
             Sq = blk.se.fc1.out_features
@@ -568,7 +598,6 @@ class MNEngine:
                               self._wgrad(du1, R["mean"], G[blk.se.fc1.weight], G[blk.se.fc1.bias], B, Sq, blk.cexp, g_code=0, a_code=0)),
                      du2, du1)
         # depthwise: BN2 + activation (+ SE gate / squeeze gradient composed on the fly)
-        sums2 = None
         if blk.se is not None and self.se_fused:
             sums2 = self._zero_pool.take(2, blk.cexp, dev)
             L.se_bn_bwd_combine(part.data_ptr(), parts, gate.data_ptr(), dpool.data_ptr(), R["sv2"][1].data_ptr(), B,
@@ -621,7 +650,7 @@ class MNEngine:
             return da1
         dev = da1.device
         Pi = R["Fi"] * R["Ti"]
-        if self.expand_bwd_fused and self.dcode == 0 and self._pw_bwd_fused_takes(B * Pi, blk.cexp, blk.cin):
+        if self.expand_bwd_fused and self.dcode == 0 and self._plan_takes("pw_bwd_plan", B * Pi, blk.cexp, blk.cin):
             # dz1 is computed on load and never stored; one pass yields the block input's gradient and the expand weight's
             coef = self._bn_bwd_coef(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
                                      G[blk.expand[1].weight], G[blk.expand[1].bias], dev, 0, sums1)
@@ -642,15 +671,16 @@ class MNEngine:
                    res=dy if blk.res else None)
         return dinp
 
-    def _pw_bwd_fused_takes(self, M, cexp, cin):
-        """whether eat_pw_conv_bwd_fused's planner accepts the expand stage (host-only, asked once per shape)"""
-        key = (M, cexp, cin)
+    def _plan_takes(self, planner, M, cexp, cn):
+        """whether the fused 1x1 backward kernel behind `planner` (pw_bwd_plan: expand stage, pw_proj_bwd_plan: project
+        stage) accepts the shape (host-only, asked once per shape)"""
+        key = (planner, M, cexp, cn)
         if key not in self._pw_bwd_ok:
             import ctypes
             from ._lib import EatError
             plan = (ctypes.c_int * 4)()
             try:
-                lib().pw_bwd_plan(M, cexp, cin, ctypes.addressof(plan))
+                getattr(lib(), planner)(M, cexp, cn, ctypes.addressof(plan))
                 self._pw_bwd_ok[key] = True
             except EatError:
                 self._pw_bwd_ok[key] = False
@@ -715,10 +745,18 @@ class MNEngine:
         St = S["stem"]
         conv, bn = self.stem[0], self.stem[1]
         c0 = conv.out_channels
-        dz0 = self._bn_bwd(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0, G[bn.weight],
-                           G[bn.bias], dev)
-        L.stem_wgrad(dz0.data_ptr(), dc, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
-                     conv.stride[0], st)
+        if self.stem_bwd_fused and dc == 0 and c0 <= 64 and c0 % 4 == 0 and conv.stride[0] in (1, 2):
+            # dz0 is computed on load in its only consumer and never stored
+            coef = self._bn_bwd_coef(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0,
+                                     G[bn.weight], G[bn.bias], dev, 0, None)
+            L.stem_wgrad(dy.data_ptr(), 0, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
+                         conv.stride[0], St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
+                         St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(), st)
+        else:
+            dz0 = self._bn_bwd(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0, G[bn.weight],
+                               G[bn.bias], dev)
+            L.stem_wgrad(dz0.data_ptr(), dc, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
+                         conv.stride[0], 0, 0, 0, 0, 0, 0, 0, 0, st)
         fork.join()
         self._fork = None
         G[None] = flat

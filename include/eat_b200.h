@@ -307,9 +307,30 @@ int eat_pw_conv_bwd_fused(const float* da, const float* z, const float* scale, c
  * EAT_ERR_ARG), and its launch on a 132-SM H100: plan[4] = {CTAs (one per SM at most, each a contiguous range of
  * 128-row tiles), rows per CTA at most, pipeline stages, dynamic shared-memory bytes}. */
 int eat_pw_bwd_plan(long long M, int cexp, int cin, int* plan);
-/* Stem weight gradient (the spectrogram itself needs no gradient). */
+/* Backward of an InvertedResidual's project stage (1x1 conv + BatchNorm, no activation) for a block without
+ * squeeze-excitation, in one pass over its tensors: from the gradient dy [M, cout] at the BatchNorm's output, its raw
+ * output z3 [M, cout] and the depthwise stage's raw output z2 [M, cexp]: dz3 = eat_bn_bwd_apply(dy, NULL, NULL, z3,
+ * scale3 ... c2, act none) is computed on load and never stored; dp [M, cexp] = dz3 . W with W the project weight
+ * [cout, cexp]; dW [cout, cexp] += dz3^T . act(z2 * scale2 + shift2) (zeroed by the caller, atomically accumulated);
+ * and the depthwise BatchNorm's backward sums s1[c] += sum g, s2[c] += invstd2[c] * sum g * (z2 - mean2[c]) with
+ * g = dp * act'(z2 * scale2 + shift2) -- what eat_bn_bwd_reduce(dp, NULL, NULL, z2, ...) adds.  c1/c2 come from
+ * eat_bn_bwd_finalize of BN3's sums.  bf16x3 tensor-core products as eat_pw_conv_bwd_fused.  fp32 storage, act relu or
+ * hardswish, cout <= 32 and cexp <= 128, both multiples of 4; anything else returns EAT_ERR_UNSUPPORTED / EAT_ERR_ARG
+ * before any launch.  M == 0 is a no-op. */
+int eat_pw_proj_bwd_fused(const float* dy, const float* z3, const float* scale3, const float* shift3, const float* mean3,
+                          const float* invstd3, const float* c1, const float* c2, const float* z2, const float* scale2,
+                          const float* shift2, const float* mean2, const float* invstd2, int act, const float* W, float* dp,
+                          float* dW, double* s1, double* s2, int dtype, long long M, int cexp, int cout,
+                          cudaStream_t stream);
+/* Host-only: whether eat_pw_proj_bwd_fused takes a shape, and its launch plan, as eat_pw_bwd_plan. */
+int eat_pw_proj_bwd_plan(long long M, int cexp, int cout, int* plan);
+/* Stem weight gradient (the spectrogram itself needs no gradient).  z == NULL: dz is the gradient at the conv output.
+ * z != NULL: dz is the gradient dy at the stem BatchNorm + activation's output and z the raw conv output, and the conv
+ * output's gradient eat_bn_bwd_apply(dy, NULL, NULL, z, scale, shift, mean, invstd, act, c1, c2) is computed on load and
+ * never stored (fp32 storage, C <= 64, stride 1 or 2; otherwise EAT_ERR_UNSUPPORTED before any launch). */
 int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, int F, int T, int C, int stride,
-                   cudaStream_t stream);
+                   const float* z, const float* scale, const float* shift, const float* mean, const float* invstd, int act,
+                   const float* c1, const float* c2, cudaStream_t stream);
 /* dpre = dh * mask * act'(pre), fp32 vectors (classifier Hardswish + Dropout backward). */
 int eat_act_bwd(const float* dh, const float* pre, const float* mask, int act, float* dpre, long long n,
                 cudaStream_t stream);
