@@ -430,9 +430,21 @@ int eat_ctx_pool(const void* x, int dtype, float* out, int B, int F, int T, int 
   return EAT_OK;
 }
 
+// shared by eat_seq_pool / eat_seq_pool_bwd: the window [row0, row0 + L) must lie inside [0, Ltot), and the pooling
+// stride must be positive (1 = copy, otherwise AvgPool(3, stride, pad 1))
+static int seq_pool_check(int B, int Ltot, int row0, int L, int H, int stride) {
+  if (stride < 1) { eat_set_error("seq_pool: stride must be at least 1"); return EAT_ERR_ARG; }
+  if (B < 0 || L < 1 || H < 1 || row0 < 0 || (long long)row0 + L > Ltot) {
+    eat_set_error("seq_pool: rows [row0, row0 + L) must lie inside [0, Ltot), with L >= 1 and H >= 1");
+    return EAT_ERR_ARG;
+  }
+  return EAT_OK;
+}
+
 int eat_seq_pool(const float* in, float* out, int B, int Ltot, int row0, int L, int H, int stride, const float* scale,
                  const float* shift, int act, cudaStream_t st) {
   if (B == 0) return EAT_OK;
+  if (int rc = seq_pool_check(B, Ltot, row0, L, H, stride)) return rc;
   const int Lo = stride == 1 ? L : (L + 2 - 3) / stride + 1;
   dim3 grid(ceil_div(Lo * H, 256), B);
   seq_pool_kernel<<<grid, 256, 0, st>>>(in, out, Ltot, row0, L, Lo, H, stride, scale, shift, act);
@@ -506,6 +518,7 @@ int eat_sigmoid_bwd(const float* g, const float* s, float* out, long long n, cud
 int eat_dyconv_att_bwd(const float* datt, const float* att, float temperature, const float* hc, const float* wr,
                        float* dwr, float* dbr, float* dhc, int B, int H, int k, cudaStream_t st) {
   if (B == 0) return EAT_OK;
+  if (k < 1 || k > 4) { eat_set_error("dyconv_att_bwd: 1..4 kernels supported"); return EAT_ERR_UNSUPPORTED; }
   dyconv_att_bwd_kernel<<<ceil_div(B, 4), 128, 0, st>>>(datt, att, 1.f / temperature, hc, wr, dwr, dbr, dhc, B, H, k);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
@@ -513,6 +526,7 @@ int eat_dyconv_att_bwd(const float* datt, const float* att, float temperature, c
 
 int eat_seq_pool_bwd(const float* dout, float* dsrc, int B, int Ltot, int row0, int L, int H, int stride, cudaStream_t st) {
   if (B == 0) return EAT_OK;
+  if (int rc = seq_pool_check(B, Ltot, row0, L, H, stride)) return rc;
   const int Lo = stride == 1 ? L : (L + 2 - 3) / stride + 1;
   dim3 grid(ceil_div(L * H, 256), B);
   seq_pool_bwd_kernel<<<grid, 256, 0, st>>>(dout, dsrc, Ltot, row0, L, Lo, H, stride);

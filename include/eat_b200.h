@@ -174,7 +174,8 @@ int eat_dw_conv_fwd_dy(const void* in, const float* wt, long long wt_bstride, vo
 /* ContextGen pooling (dy_block.py:236-240): out [B, F+T, C] fp32 = [mean over T | mean over F]. */
 int eat_ctx_pool(const void* x, int dtype, float* out, int B, int F, int T, int C, cudaStream_t stream);
 /* Sequence pooling of ContextGen (dy_block.py:227-233,249): AvgPool(3, stride, pad 1) or copy (stride 1) of rows
- * [row0, row0+L) of each sample of in [B, Ltot, H] -> out [B, Lo, H]. */
+ * [row0, row0+L) of each sample of in [B, Ltot, H] -> out [B, Lo, H].  stride >= 1 and row0 + L <= Ltot, else EAT_ERR_ARG
+ * (also for eat_seq_pool_bwd). */
 int eat_seq_pool(const float* in, float* out, int B, int Ltot, int row0, int L, int H, int stride, const float* scale,
                  const float* shift, int act, cudaStream_t stream);   /* optional affine+act applied to `in` on load */
 /* att [B,k] = softmax((Wr h_c + br)/temperature)  (dy_block.py:104-107). */
@@ -195,7 +196,7 @@ int eat_dy_act_bwd(const void* dp, const void* z, void* du, int dtype, const flo
 int eat_dyrelu_coef_bwd(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n,
                         cudaStream_t stream);
 int eat_sigmoid_bwd(const float* g, const float* s, float* out, long long n, cudaStream_t stream);
-/* softmax(Linear(h_c)/T) backward: dWr/dbr accumulated, dh_c[b,:] += dlogit . Wr. */
+/* softmax(Linear(h_c)/T) backward: dWr/dbr accumulated, dh_c[b,:] += dlogit . Wr.  k in 1..4, as eat_dyconv_att. */
 int eat_dyconv_att_bwd(const float* datt, const float* att, float temperature, const float* hc, const float* wr,
                        float* dwr, float* dbr, float* dhc, int B, int H, int k, cudaStream_t stream);
 int eat_seq_pool_bwd(const float* dout, float* dsrc, int B, int Ltot, int row0, int L, int H, int stride,

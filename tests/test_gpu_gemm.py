@@ -216,7 +216,9 @@ def test_tma_dynamic_gemm_matches_per_sample_reference(w_trans):
     st = torch.cuda.current_stream().cuda_stream
     p = lambda t: 0 if t is None else t.data_ptr()
     for idx, (B, rps, N, K) in enumerate([(3, 500, 64, 16), (2, 2000, 24, 72), (5, 130, 200, 80), (4, 128, 112, 672), (2, 63, 8, 8),
-                                          (3, 504, 960, 160), (7, 37, 40, 120)]):
+                                          (3, 504, 960, 160), (7, 37, 40, 120),
+                                          # B >= 8: several samples' tiles per CTA, per-sample kernels past the first eight
+                                          (12, 101, 64, 16), (64, 28, 24, 72)]):
         M, nk = B * rps, 4
         A = torch.randn(M, K, device="cuda", generator=g)
         W = torch.randn(nk, N, K, device="cuda", generator=g) / K ** 0.5
