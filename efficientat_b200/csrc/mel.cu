@@ -1,30 +1,56 @@
-// Fused log-mel front end: pre-emphasis + reflect pad + framing + window + 1024-pt real FFT in
+// Fused log-mel front end: pre-emphasis + reflect pad + framing + window + n_fft-point real FFT in
 // shared memory + power + banded mel filterbank + log + affine.   One kernel, waveform in,
 // normalised log-mel out.  Replaces reference models/preprocess.py:40-67 (eval path; the
 // fmin/fmax jitter of the training path only changes the filterbank table passed in).
 //
-// Work decomposition: grid = (ceil(T / 16), B).  A CTA owns 16 consecutive frames of one clip: it stages its slice of the
-// pre-emphasised, reflect-padded signal in shared memory once (round 2; the frames overlap by n_fft - hop samples), then
-// 256 threads = 4 independent groups of 64 (group-local named barriers) transform one frame each per round (512-point
-// complex FFT as three radix-8 Stockham passes, 8 complex values per thread in registers), 4 rounds.
-// Results are staged in shared memory as [n_mels][16] so the global store is 64 B per mel row.
-// Algorithmic HBM bytes: 4*N read + 4*n_mels*T written per clip (1.792 MB at 10 s / 32 kHz).
+// n_fft is a power of two in [256, 4096]; mel_kernel<M> is instantiated per complex FFT length M = n_fft / 2.
+// Work decomposition: grid = (ceil(T / F), B).  A CTA owns F consecutive frames of one clip: it stages its slice of the
+// pre-emphasised, reflect-padded signal in shared memory once (the frames overlap by n_fft - hop samples), then its
+// 256 threads, as independent groups of M/8 (group-local barriers), transform one frame per group and round: M-point
+// complex FFT as floor(log8 M) radix-8 Stockham passes plus one radix-2/4 pass when log2 M is not a multiple of 3,
+// 8 complex values per thread in registers.
+//
+//   n_fft   M     passes    threads/group  groups  F (frames/CTA)  rounds
+//   256     128   8·8·2     16             16      16              1
+//   512     256   8·8·4     32             8       16              2
+//   1024    512   8·8·8     64             4       16              4
+//   2048    1024  8·8·8·2   128            2       16              8
+//   4096    2048  8·8·8·4   256            1       8               8
+//
+// Results are staged in shared memory as [n_mels][F] so the global store is 4·F bytes per mel row.
+// Algorithmic HBM bytes: 4*N read + 4*n_mels*T written per clip (1.792 MB at 10 s / 32 kHz / hop 320 / 128 mels).
 #include "common.cuh"
 #include "fft_core.cuh"
 #include <math.h>
 
 namespace {
 
-constexpr int kNfft = 1024;
-constexpr int kHalf = 512;          // complex FFT length
-constexpr int kFramesPerCta = 16;
-constexpr int kGroups = 4;
 constexpr int kThreads = 256;
+constexpr size_t kSmemCap = 227 * 1024;     // opt-in shared memory per block on sm_90
+
+template <int M>
+struct MelShape {
+  static_assert(M >= 128 && M <= 2048 && (M & (M - 1)) == 0, "complex FFT length: a power of two in [128, 2048]");
+  static constexpr int kNfft = 2 * M;
+  static constexpr int kGroupThreads = M / 8;                     // one radix-8 work item per thread
+  static constexpr int kGroups = kThreads / kGroupThreads;
+  static constexpr int kFrames = M == 2048 ? 8 : 16;             // frames per CTA; 8 at n_fft 4096 keeps long hops
+                                                                  // within shared memory next to the 48 KB of tables
+  static constexpr int kPow = M + 4;                              // power bins 0..M, padded to 16 B
+  static constexpr int kLog2 = M == 128 ? 7 : M == 256 ? 8 : M == 512 ? 9 : M == 1024 ? 10 : 11;
+  static constexpr int kLog2Group = kLog2 - 3;
+  static constexpr int kRadix8End = kLog2 >= 9 ? 512 : 64;        // radix-8 passes run at Ns = 1, 8 (, 64)
+  static constexpr int kTail = kLog2 % 3 == 0 ? 1 : kLog2 % 3 == 1 ? 2 : 4;   // radix of the last pass, 1 = none
+  static_assert(kFrames % kGroups == 0, "whole rounds");
+  // bytes that do not depend on the geometry: twiddles, window, per-group FFT and power buffers
+  static constexpr size_t kSmemFixed = kNfft * sizeof(float2) + kNfft * sizeof(float) +
+                                       kGroups * (M * sizeof(float2) + kPow * sizeof(float));
+};
 
 struct MelParams {
   const float* wave;     // [B, N]
   const float* window;   // [win_length]
-  const float2* twiddle; // [512] exp(-2 pi i m/512) followed by [512] exp(-2 pi i k/1024)
+  const float2* twiddle; // [M] exp(-2 pi i m/M) followed by [M] exp(-2 pi i k/n_fft), M = n_fft / 2
   const int* fb_start;   // [n_mels] first FFT bin of each filter
   const int* fb_len;     // [n_mels] number of taps
   const float* fb_w;     // [max_len][n_mels] taps, tap-major
@@ -45,29 +71,42 @@ __device__ __forceinline__ float preemph_sample(const float* __restrict__ x, int
   return __ldg(x + q + 1) - c * __ldg(x + q);
 }
 
-__device__ __forceinline__ void group_sync(int grp) {       // the four 64-thread groups work on different frames: no CTA barrier
-  asm volatile("bar.sync %0, 64;" ::"r"(grp + 1) : "memory");
+// the groups of a CTA work on different frames: no CTA barrier.  bar.sync takes thread counts that are multiples
+// of 32 and a CTA has 16 barrier ids, so groups of one warp (n_fft 512) or half a warp (n_fft 256) use __syncwarp
+template <int G>
+__device__ __forceinline__ void group_sync(int grp) {
+  static_assert(G == 16 || G % 32 == 0, "group size");
+  if constexpr (G >= 64) {
+    asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "n"(G) : "memory");
+  } else if constexpr (G == 32) {
+    __syncwarp();
+  } else {
+    __syncwarp(0xffffu << (16 * (grp & 1)));
+  }
 }
 
+template <int M>
 __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
+  using S = MelShape<M>;
+  constexpr int G = S::kGroupThreads, F = S::kFrames, NF = S::kNfft;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  float2* s_tw = reinterpret_cast<float2*>(smem_raw);                 // 1024 float2  (8 KB)
-  float* s_win = reinterpret_cast<float*>(s_tw + 1024);               // 1024 floats  (4 KB) zero-padded window
-  float2* s_fft = reinterpret_cast<float2*>(s_win + kNfft);           // kGroups * 512 float2 (16 KB)
-  float* s_pow = reinterpret_cast<float*>(s_fft + kGroups * kHalf);   // kGroups * 516 floats
-  float* s_out = s_pow + kGroups * 516;                               // n_mels * (kFramesPerCta + 1) floats
-  float* s_sig = s_out + p.n_mels * (kFramesPerCta + 1);              // seg_len floats: the CTA's slice of the signal
+  float2* s_tw = reinterpret_cast<float2*>(smem_raw);                 // n_fft float2
+  float* s_win = reinterpret_cast<float*>(s_tw + NF);                 // n_fft floats, zero-padded window
+  float2* s_fft = reinterpret_cast<float2*>(s_win + NF);              // kGroups * M float2
+  float* s_pow = reinterpret_cast<float*>(s_fft + S::kGroups * M);    // kGroups * (M + 4) floats
+  float* s_out = s_pow + S::kGroups * S::kPow;                        // n_mels * (F + 1) floats
+  float* s_sig = s_out + p.n_mels * (F + 1);                          // seg_len floats: the CTA's slice of the signal
 
   const int tid = threadIdx.x;
-  const int grp = tid >> 6;
-  const int j = tid & 63;
+  const int grp = tid >> S::kLog2Group;
+  const int j = tid & (G - 1);
   const int b = blockIdx.y;
-  const int t_base = blockIdx.x * kFramesPerCta;
+  const int t_base = blockIdx.x * F;
   const float* __restrict__ x = p.wave + (size_t)b * p.N;
   const int L = p.N - 1;
-  const int lp = (kNfft - p.win_length) / 2;
+  const int lp = (NF - p.win_length) / 2;
 
-  for (int i = tid; i < 1024; i += kThreads) {
+  for (int i = tid; i < NF; i += kThreads) {
     s_tw[i] = p.twiddle[i];
     int wi = i - lp;
     s_win[i] = (wi >= 0 && wi < p.win_length) ? p.window[wi] : 0.f;
@@ -75,77 +114,106 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
   // pre-emphasis + reflection once per sample (coalesced), instead of 32 scalar global loads per thread and frame:
   // neighbouring frames overlap by n_fft - hop samples
   {
-    const int s0 = t_base * p.hop - kHalf;
+    const int s0 = t_base * p.hop - M;
     for (int i = tid; i < p.seg_len; i += kThreads) s_sig[i] = preemph_sample(x, s0 + i, L, p.preemph);
   }
   __syncthreads();
 
-  float2* zf = s_fft + grp * kHalf;
-  float* pw = s_pow + grp * 516;
+  float2* zf = s_fft + grp * M;
+  float* pw = s_pow + grp * S::kPow;
 
-  for (int round = 0; round < kFramesPerCta / kGroups; ++round) {
-    const int fl = round * kGroups + grp;     // frame index inside the CTA tile
+  for (int round = 0; round < F / S::kGroups; ++round) {
+    const int fl = round * S::kGroups + grp;   // frame index inside the CTA tile
     const int t = t_base + fl;
-    const bool live = t < p.T;                // uniform within a group
+    const bool live = t < p.T;                 // uniform within a group
     float2 v[8];
     // ---- pass 1 (Ns = 1): window the staged samples
     if (live) {
       const float* sg = s_sig + fl * p.hop;
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
-        const int n = j + 64 * r;
+        const int n = j + G * r;
         v[r] = make_float2(s_win[2 * n] * sg[2 * n], s_win[2 * n + 1] * sg[2 * n + 1]);
       }
-      stockham8_compute(v, j, 1, s_tw);
+      stockham8_compute_m(v, j, 1, M, s_tw);
 #pragma unroll
       for (int r = 0; r < 8; ++r) zf[stockham8_dst(j, 1, r)] = v[r];
     }
-    group_sync(grp);
-    // ---- pass 2 (Ns = 8), pass 3 (Ns = 64), in place with a barrier between gather and scatter
+    group_sync<G>(grp);
+    // ---- the other radix-8 passes (Ns = 8 (, 64)), in place with a barrier between gather and scatter
 #pragma unroll
-    for (int Ns = 8; Ns <= 64; Ns *= 8) {
+    for (int Ns = 8; Ns < S::kRadix8End; Ns *= 8) {
       if (live) {
 #pragma unroll
-        for (int r = 0; r < 8; ++r) v[r] = zf[j + 64 * r];
-        stockham8_compute(v, j, Ns, s_tw);
+        for (int r = 0; r < 8; ++r) v[r] = zf[j + G * r];
+        stockham8_compute_m(v, j, Ns, M, s_tw);
       }
-      group_sync(grp);
+      group_sync<G>(grp);
       if (live) {
 #pragma unroll
         for (int r = 0; r < 8; ++r) zf[stockham8_dst(j, Ns, r)] = v[r];
       }
-      group_sync(grp);
+      group_sync<G>(grp);
     }
-    // ---- real-FFT split + power spectrum, bins 0..512
+    // ---- radix-2 / radix-4 tail: every thread writes back exactly the slots it read
+    if constexpr (S::kTail != 1) {
+      if (live) {
+#pragma unroll
+        for (int r = 0; r < 8; ++r) v[r] = zf[j + G * r];
+        if constexpr (S::kTail == 2) stockham2_tail(v, j, M, s_tw);
+        else stockham4_tail(v, j, M, s_tw);
+#pragma unroll
+        for (int r = 0; r < 8; ++r) zf[j + G * r] = v[r];
+      }
+      group_sync<G>(grp);
+    }
+    // ---- real-FFT split + power spectrum, bins 0..M
     if (live) {
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
-        int k = j + 64 * r;
-        float2 X = rfft_split(zf[k], zf[(kHalf - k) & (kHalf - 1)], s_tw[512 + k]);
+        int k = j + G * r;
+        float2 X = rfft_split(zf[k], zf[(M - k) & (M - 1)], s_tw[M + k]);
         pw[k] = X.x * X.x + X.y * X.y;
       }
-      if (j == 0) { float2 z0 = zf[0]; float nyq = z0.x - z0.y; pw[512] = nyq * nyq; }
+      if (j == 0) { float2 z0 = zf[0]; float nyq = z0.x - z0.y; pw[M] = nyq * nyq; }
     }
-    group_sync(grp);
+    group_sync<G>(grp);
     // ---- banded mel + log + affine into the staging tile
     if (live) {
-      for (int m = j; m < p.n_mels; m += 64) {
+      for (int m = j; m < p.n_mels; m += G) {
         int st = __ldg(p.fb_start + m), len = __ldg(p.fb_len + m);
         float acc = 0.f;
         for (int i = 0; i < len; ++i) acc = fmaf(__ldg(p.fb_w + (size_t)i * p.n_mels + m), pw[st + i], acc);
-        s_out[m * (kFramesPerCta + 1) + fl] = (logf(acc + p.log_offset) + p.out_add) / p.out_div;
+        s_out[m * (F + 1) + fl] = (logf(acc + p.log_offset) + p.out_add) / p.out_div;
       }
     }
-    group_sync(grp);                          // zf / pw are rewritten by this group's next round
+    group_sync<G>(grp);                         // zf / pw are rewritten by this group's next round
   }
   __syncthreads();
-  // ---- store: 16 consecutive frames (64 bytes) of one mel row per half warp
+  // ---- store: F consecutive frames (4·F bytes) of one mel row per F lanes, 32 / F mel rows per warp instruction
   const int lane = tid & 31, warp = tid >> 5;
-  const int fo = lane & (kFramesPerCta - 1), sub = lane / kFramesPerCta;       // two mel rows per warp instruction
+  const int fo = lane & (F - 1), sub = lane / F;
   const int t = t_base + fo;
-  for (int m = warp * 2 + sub; m < p.n_mels; m += (kThreads / 32) * 2) {
-    if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = s_out[m * (kFramesPerCta + 1) + fo];
+  for (int m = warp * (32 / F) + sub; m < p.n_mels; m += (kThreads / 32) * (32 / F)) {
+    if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = s_out[m * (F + 1) + fo];
   }
+}
+
+template <int M>
+int mel_launch(MelParams p, cudaStream_t stream) {
+  using S = MelShape<M>;
+  const long long seg_len = (long long)(S::kFrames - 1) * p.hop + S::kNfft;
+  const size_t smem = S::kSmemFixed + ((size_t)p.n_mels * (S::kFrames + 1) + (size_t)seg_len) * sizeof(float);
+  if (smem > kSmemCap) {
+    eat_set_error("eat_mel_fwd: hop too large for the shared-memory signal slice"); return EAT_ERR_UNSUPPORTED;
+  }
+  p.seg_len = (int)seg_len;
+  static unsigned long long attr_mask = 0;
+  if (int rc = eat_opt_in_smem(mel_kernel<M>, kSmemCap, attr_mask)) return rc;
+  dim3 grid(ceil_div(p.T, S::kFrames), p.B);
+  mel_kernel<M><<<grid, kThreads, smem, stream>>>(p);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
 }
 
 // training-time SpecAugment bands (torchaudio Frequency/TimeMasking, iid per example): positions inside
@@ -218,7 +286,9 @@ extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window,
                            int n_fft, const float* twiddle, const int* fb_start, const int* fb_len,
                            const float* fb_w, int max_len, int n_mels, float preemph, float* out,
                            cudaStream_t stream) {
-  if (n_fft != kNfft) { eat_set_error("eat_mel_fwd: only n_fft == 1024 is implemented"); return EAT_ERR_UNSUPPORTED; }
+  if (n_fft != 256 && n_fft != 512 && n_fft != 1024 && n_fft != 2048 && n_fft != 4096) {
+    eat_set_error("eat_mel_fwd: n_fft must be one of 256, 512, 1024, 2048, 4096"); return EAT_ERR_UNSUPPORTED;
+  }
   if (win_length > n_fft || win_length < 1 || hop < 1 || n_mels < 1 || n_mels > 512 || B < 0) {
     eat_set_error("eat_mel_fwd: bad geometry"); return EAT_ERR_ARG;
   }
@@ -229,15 +299,11 @@ extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window,
   p.fb_start = fb_start; p.fb_len = fb_len; p.fb_w = fb_w; p.out = out;
   p.B = B; p.N = N; p.T = 1 + (N - 1) / hop; p.n_mels = n_mels; p.win_length = win_length; p.hop = hop;
   p.max_len = max_len; p.preemph = preemph; p.log_offset = 1e-5f; p.out_add = 4.5f; p.out_div = 5.f;
-  p.seg_len = (kFramesPerCta - 1) * hop + kNfft;
-  size_t smem = 1024 * sizeof(float2) + kNfft * sizeof(float) + kGroups * kHalf * sizeof(float2) +
-                kGroups * 516 * sizeof(float) + (size_t)n_mels * (kFramesPerCta + 1) * sizeof(float) +
-                (size_t)p.seg_len * sizeof(float);
-  if (smem > 160 * 1024) { eat_set_error("eat_mel_fwd: hop too large for the shared-memory signal slice"); return EAT_ERR_UNSUPPORTED; }
-  static unsigned long long attr_mask = 0;
-  if (int rc = eat_opt_in_smem(mel_kernel, 160 * 1024, attr_mask)) return rc;
-  dim3 grid(ceil_div(p.T, kFramesPerCta), B);
-  mel_kernel<<<grid, kThreads, smem, stream>>>(p);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  switch (n_fft) {
+    case 256: return mel_launch<128>(p, stream);
+    case 512: return mel_launch<256>(p, stream);
+    case 1024: return mel_launch<512>(p, stream);
+    case 2048: return mel_launch<1024>(p, stream);
+    default: return mel_launch<2048>(p, stream);
+  }
 }

@@ -61,10 +61,12 @@ class AugmentMelSTFT(nn.Module):
         self.register_buffer("preemphasis_coefficient", torch.as_tensor([[[-.97, 1]]]), persistent=False)
         self.freqm = nn.Identity() if freqm == 0 else _AxisMasking(freqm, 1)
         self.timem = nn.Identity() if timem == 0 else _AxisMasking(timem, 2)
-        # FFT twiddles in fp64 -> fp32: exp(-2 pi i m / 512), m < 512, then exp(-2 pi i k / 1024), k < 512
-        m = torch.arange(512, dtype=torch.float64)
-        tw = torch.cat([torch.stack([torch.cos(2 * math.pi * m / 512), -torch.sin(2 * math.pi * m / 512)], 1),
-                        torch.stack([torch.cos(2 * math.pi * m / 1024), -torch.sin(2 * math.pi * m / 1024)], 1)])
+        # FFT twiddles in fp64 -> fp32, with M = n_fft / 2: exp(-2 pi i m / M), m < M, then exp(-2 pi i k / n_fft), k < M.
+        # The kernel takes n_fft in {256, 512, 1024, 2048, 4096}; any other value raises EatError at the first forward.
+        half = n_fft // 2
+        m = torch.arange(half, dtype=torch.float64)
+        tw = torch.cat([torch.stack([torch.cos(2 * math.pi * m / half), -torch.sin(2 * math.pi * m / half)], 1),
+                        torch.stack([torch.cos(2 * math.pi * m / n_fft), -torch.sin(2 * math.pi * m / n_fft)], 1)])
         self.register_buffer("_twiddle", tw.float().contiguous(), persistent=False)
         self._fb_cache = {}
         self._preemph = 0.97      # value of preemphasis_coefficient[0,0,0] negated (preprocess.py:30)

@@ -58,9 +58,11 @@ int eat_device_check(int device);
 
 /* Fused log-mel front end.  Replaces AugmentMelSTFT.forward, models/preprocess.py:40-67
  * (conv1d pre-emphasis :41, torch.stft :42-43, power :44, mel matmul :56-57, log :59, affine :65).
- * wave [B,N] fp32 -> out [B, n_mels, 1+(N-1)/hop] fp32.  twiddle: 1024 float2 (exp(-2 pi i m/512),
- * m<512, then exp(-2 pi i k/1024), k<512).  Filterbank as bands: fb_start/fb_len [n_mels],
- * fb_w [max_len][n_mels] (tap-major). */
+ * wave [B,N] fp32 -> out [B, n_mels, 1+(N-1)/hop] fp32.  n_fft in {256, 512, 1024, 2048, 4096}, anything
+ * else returns EAT_ERR_UNSUPPORTED; win_length <= n_fft, n_mels <= 512, N - 1 > n_fft/2, else EAT_ERR_ARG; a hop
+ * whose signal slice does not fit in shared memory returns EAT_ERR_UNSUPPORTED.  All checks precede any device call.
+ * twiddle: n_fft float2 (exp(-2 pi i m/M), m<M, then exp(-2 pi i k/n_fft), k<M, with M = n_fft/2).
+ * Filterbank as bands: fb_start/fb_len [n_mels], fb_w [max_len][n_mels] (tap-major). */
 int eat_mel_fwd(const float* wave, int B, int N, const float* window, int win_length, int hop, int n_fft,
                 const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len,
                 int n_mels, float preemph, float* out, cudaStream_t stream);
