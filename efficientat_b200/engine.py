@@ -18,6 +18,8 @@ import os
 import torch
 
 from ._lib import check_module_tensors, lib
+from .models.common import head_dropout
+from .models.mn.attention_pooling import MultiHeadAttentionPooling
 
 ACT = {"none": 0, "relu": 1, "hswish": 2}
 BN_EPS = 1e-3
@@ -118,6 +120,8 @@ class _Fork:
 
 
 class MNEngine:
+    mha = None          # the MultiHeadAttentionPooling classifier, when the model has that head instead of 'mlp' (see _plan)
+
     def __init__(self, model):
         self.model = model
         self.precision = getattr(model, "precision", "fp32")
@@ -179,9 +183,11 @@ class MNEngine:
             L.stride = m.cnf.stride
             L.cin, L.cexp, L.cout = m.cnf.input_channels, m.cnf.expanded_channels, m.cnf.out_channels
             self.blocks.append(L)
-        self.fc1 = self.model.classifier[2]
-        self.fc2 = self.model.classifier[5]
-        self.dropout_p = self.model.classifier[4].p
+        self.mha = self.model.classifier if isinstance(self.model.classifier, MultiHeadAttentionPooling) else None
+        if self.mha is None:
+            self.fc1 = self.model.classifier[2]
+            self.fc2 = self.model.classifier[5]
+        self.dropout_p = head_dropout(self.model)
 
     @property
     def tdtype(self):
@@ -272,7 +278,7 @@ class MNEngine:
         if x.dim() != 4 or x.shape[1] != 1:
             raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
         check_module_tensors(self.model, x.device, type(self.model).__name__)
-        self.dropout_p = float(self.model.classifier[4].p)          # read at call time (it may be changed after engine())
+        self.dropout_p = head_dropout(self.model)                    # read at call time (it may be changed after engine())
         needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.model.parameters())
         with torch.cuda.device(x.device):                            # launches go to x's device, whatever is current
             if self.model.training:
@@ -360,6 +366,9 @@ class MNEngine:
         M = B * Fi * Ti
         z = torch.empty(B, Fi, Ti, cl, device=dev, dtype=td)
         self._gemm(a, conv.weight, z, M, cl, conv.in_channels, sc=self._fold(bn, dev), act=ACT["hswish"])
+        if self.mha is not None:
+            logits, feat, _ = self._mha_fwd(z, None, B, Fi, Ti, save=False)
+            return logits, feat, z
         feat = torch.zeros(B, cl, device=dev, dtype=torch.float32)
         L.bn_act_pool(z.data_ptr(), 0, 0, 0, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B, Fi * Ti, cl, st)
         h = torch.empty(B, self.fc1.out_features, device=dev, dtype=torch.float32)
@@ -465,10 +474,13 @@ class MNEngine:
         stt = self._new_stats(cl, dev)
         self._gemm(a, conv.weight, zl, M, cl, conv.in_channels, stats=stt)
         scl, svl = self._finalize(bn, stt, M, dev)
+        S["last"] = dict(inp=a, z=zl, sc=scl, sv=svl, Fi=Fi, Ti=Ti)
+        if self.mha is not None:
+            logits, feat, S["head"] = self._mha_fwd(zl, scl, B, Fi, Ti, save=True)
+            return logits, feat
         feat = torch.zeros(B, cl, device=dev, dtype=torch.float32)
         L.bn_act_pool(zl.data_ptr(), scl[0].data_ptr(), scl[1].data_ptr(), HS, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B,
                       Fi * Ti, cl, st)
-        S["last"] = dict(inp=a, z=zl, sc=scl, sv=svl, Fi=Fi, Ti=Ti)
         # classifier: Linear -> Hardswish -> Dropout -> Linear.  The Hardswish and the dropout mask are applied on
         # the operand load of the second GEMM (in_act + per-row gate), so only the pre-activation is stored.
         n1 = self.fc1.out_features
@@ -483,6 +495,50 @@ class MNEngine:
                    gate=dropout_mask, rows_per_sample=1, bias=self.fc2.bias, a_code=0, c_code=0)
         S["head"] = dict(feat=feat, h_pre=h_pre, mask=dropout_mask, ident=ident)
         return logits, feat
+
+    def _mha_fwd(self, z, sc, B, Fi, Ti, save):
+        """multi-head attention pooling head (attention_pooling.py:40-56) on the last conv's output z [B, F, T, C]:
+        frequency mean (with the BatchNorm + Hardswish applied on load when sc is given, i.e. z is raw), projection GEMM,
+        attention pooling.  -> (logits [B, K], features [B, C], tensors the backward needs or None)"""
+        L = lib()
+        dev, st = z.device, _stream()
+        head = self.mha
+        C, H, K = z.shape[3], head.num_heads, head.out_dim
+        m = torch.empty(B, Ti, C, device=dev, dtype=torch.float32)
+        feat = torch.empty(B, C, device=dev, dtype=torch.float32)
+        L.freq_pool(z.data_ptr(), self.dcode, _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0,
+                    ACT["hswish"] if sc is not None else 0, m.data_ptr(), feat.data_ptr(), B, Fi, Ti, C, st)
+        P = torch.empty(B * Ti, 2 * H * K, device=dev, dtype=torch.float32)
+        proj = head.subspace_proj
+        self._gemm(m, proj.weight, P, B * Ti, 2 * H * K, C, bias=proj.bias, a_code=0, c_code=0)
+        logits = torch.empty(B, K, device=dev, dtype=torch.float32)
+        sa = r = None
+        if save:
+            sa = torch.empty(B, H, K, device=dev, dtype=torch.float32)
+            r = torch.empty_like(sa)
+        L.att_pool_fwd(P.data_ptr(), head.head_weight.data_ptr(), head.epsilon, logits.data_ptr(), _ptr(sa), _ptr(r), B, Ti,
+                       H, K, st)
+        return logits, feat, (dict(feat=feat, m=m, P=P, sa=sa, r=r) if save else None)
+
+    def _mha_bwd(self, S, dlogits, G, fork):
+        """backward of _mha_fwd down to the gradient at the last conv's BatchNorm + Hardswish output [B, F, T, C]
+        (storage dtype); parameter gradients into G"""
+        L = lib()
+        dev, st = dlogits.device, _stream()
+        head, Hd, Ls = self.mha, S["head"], S["last"]
+        B, Fi, Ti = S["B"], Ls["Fi"], Ls["Ti"]
+        C, H, K = Ls["z"].shape[3], head.num_heads, head.out_dim
+        proj = head.subspace_proj
+        dP = Hd["P"]                    # overwritten in place: P is not needed after this launch
+        L.att_pool_bwd(dlogits.data_ptr(), Hd["P"].data_ptr(), dP.data_ptr(), head.head_weight.data_ptr(),
+                       Hd["sa"].data_ptr(), Hd["r"].data_ptr(), head.epsilon, G[head.head_weight].data_ptr(),
+                       G[proj.bias].data_ptr(), B, Ti, H, K, st)
+        fork.run(lambda: self._wgrad(dP, Hd["m"], G[proj.weight], None, B * Ti, 2 * H * K, C, g_code=0, a_code=0), dP)
+        dm = torch.empty(B, Ti, C, device=dev, dtype=torch.float32)
+        self._gemm(dP, proj.weight, dm, B * Ti, C, 2 * H * K, a_code=0, c_code=0, w_trans=True)
+        gA = torch.empty_like(Ls["z"])
+        L.freq_pool_bwd(dm.data_ptr(), 1.0 / Fi, gA.data_ptr(), self.dcode, B, Fi, Ti, C, st)
+        return gA
 
     def _ident(self, n, dev):
         t = torch.empty(2, n, device=dev, dtype=torch.float32)
@@ -713,6 +769,15 @@ class MNEngine:
                 on_ready(flat, min(pidx[id(p)] for p in module.parameters()))
 
         # ---- classifier
+        Ls = S["last"]
+        P = Ls["Fi"] * Ls["Ti"]
+        conv, bn = self.last[0], self.last[1]
+        if self.mha is not None:
+            gA = self._mha_bwd(S, dlogits, G, fork)
+            done(self.model.classifier)
+            dz = self._bn_bwd(gA, None, None, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, conv.out_channels, G[bn.weight],
+                              G[bn.bias], dev)
+            return self._backward_trunk(S, G, flat, fork, done, dz)
         H = S["head"]
         n1, ncls, cl = self.fc1.out_features, self.fc2.out_features, self.fc1.in_features
         fork.run(lambda: self._wgrad(dlogits, H["h_pre"], G[self.fc2.weight], G[self.fc2.bias], B, ncls, n1, in_sc=H["ident"],
@@ -727,11 +792,22 @@ class MNEngine:
         done(self.fc1)
 
         # ---- last 1x1 conv (+BN+Hardswish, global average pool)
-        Ls = S["last"]
-        P = Ls["Fi"] * Ls["Ti"]
-        conv, bn = self.last[0], self.last[1]
         dpool = dfeat.mul_(1.0 / P)      # gradient of the spatial mean, broadcast inside the BN-backward kernels
         dz = self._bn_bwd(None, None, dpool, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, cl, G[bn.weight], G[bn.bias], dev)
+        return self._backward_trunk(S, G, flat, fork, done, dz)
+
+    def _backward_trunk(self, S, G, flat, fork, done, dz):
+        """from the gradient dz at the last 1x1 conv's output down to the stem"""
+        L = lib()
+        st = _stream()
+        dev = dz.device
+        dc = self.dcode
+        B = S["B"]
+        HS = ACT["hswish"]
+        Ls = S["last"]
+        P = Ls["Fi"] * Ls["Ti"]
+        conv = self.last[0]
+        cl = conv.out_channels
         fork.run(lambda: self._wgrad(dz, Ls["inp"], G[conv.weight], None, B * P, cl, conv.in_channels), dz)
         dy = torch.empty_like(Ls["inp"])
         self._gemm(dz, conv.weight, dy, B * P, conv.in_channels, cl, w_trans=True)

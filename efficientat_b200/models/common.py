@@ -62,10 +62,17 @@ def reference_init_(model):
             nn.init.zeros_(m.bias)
 
 
-def check_head(head_type):
-    if head_type == "mlp":
+def head_dropout(model):
+    """dropout rate of the classifier: the 'mlp' head's nn.Dropout (classifier.4); heads without dropout give 0"""
+    return float(model.classifier[4].p) if isinstance(model.classifier, nn.Sequential) else 0.0
+
+
+def check_head(head_type, supported=("mlp",)):
+    """supported: the heads the calling model implements (MN adds 'multihead_attention_pooling'; DyMN, like the reference
+    (dymn/model.py:140-142), has only 'mlp' and 'fully_convolutional')"""
+    if head_type in supported:
         return
-    if head_type in ("fully_convolutional", "multihead_attention_pooling"):
+    if head_type in ("mlp", "fully_convolutional", "multihead_attention_pooling"):
         raise NotImplementedError(f"head_type '{head_type}' is not implemented by the fused engine "
                                   "(every released *_as checkpoint used by the benchmarks has the 'mlp' head)")
     raise NotImplementedError(f"Head '{head_type}' unknown. Must be one of: 'mlp', 'fully_convolutional', "

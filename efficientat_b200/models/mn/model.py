@@ -14,6 +14,7 @@ from torch import Tensor, nn
 from torch.hub import load_state_dict_from_url
 
 from ..common import check_head, check_setting, mlp_head, reference_init_, v3_large_rows
+from ..mn.attention_pooling import MultiHeadAttentionPooling
 from ..mn.block_types import ConvNormActivation, InvertedResidual, InvertedResidualConfig
 from ..mn.utils import cnn_out_size
 
@@ -49,7 +50,7 @@ class MN(nn.Module):
         super().__init__()
         check_setting(inverted_residual_setting, InvertedResidualConfig)
         self.head_type = kwargs.get("head_type", False)
-        check_head(self.head_type)
+        check_head(self.head_type, supported=("mlp", "multihead_attention_pooling"))
         if in_conv_kernel != 3 or in_channels != 1:
             raise NotImplementedError("the fused stem kernel implements a 3x3 convolution on 1 input channel")
         make_block = InvertedResidual if block is None else block
@@ -68,7 +69,11 @@ class MN(nn.Module):
         layers.append(ConvNormActivation(last.out_channels, 6 * last.out_channels, kernel_size=1, norm_layer=bn,
                                          activation_layer=nn.Hardswish))
         self.features = nn.Sequential(*layers)
-        self.classifier = mlp_head(6 * last.out_channels, last_channel, num_classes, dropout)
+        if self.head_type == "multihead_attention_pooling":                          # mn/model.py:170-172
+            self.classifier = MultiHeadAttentionPooling(6 * last.out_channels, num_classes,
+                                                        num_heads=kwargs.get("multihead_attention_heads"))
+        else:
+            self.classifier = mlp_head(6 * last.out_channels, last_channel, num_classes, dropout)
         reference_init_(self)
         self._engine = None
         # 'fp32' keeps activations in fp32 (tensor-core bf16x3 / exact fp32 CUDA-core math, logits within 1e-3 of
@@ -102,12 +107,23 @@ def _mobilenet_v3(inverted_residual_setting, last_channel, pretrained_name, **kw
     if pretrained_name in pretrained_models:                                        # mn/model.py:282-310
         url = pretrained_models.get(pretrained_name)
         state_dict = load_state_dict_from_url(url, model_dir=model_dir, map_location="cpu")
-        num_classes = state_dict["classifier.5.bias"].size(0)
+        # the released checkpoints have the 'mlp' head; for any other head the reference looks up the keys of the
+        # 'fully_convolutional' one and raises KeyError (mn/model.py:287-302), and so does this branch
+        if kwargs["head_type"] == "mlp":
+            num_classes = state_dict["classifier.5.bias"].size(0)
+        else:
+            print("Loading weights for classifier only implemented for head types 'mlp' and 'fully_convolutional'")
+            num_classes = -1
         if kwargs["num_classes"] != num_classes:
+            pretrain_logits = state_dict["classifier.5.bias"].size(0) if kwargs["head_type"] == "mlp" \
+                else state_dict["classifier.1.bias"].size(0)
             print(f"Number of classes defined: {kwargs['num_classes']}, "
-                  f"but try to load pre-trained layer with logits: {num_classes}\nDropping last layer.")
-            del state_dict["classifier.5.weight"]
-            del state_dict["classifier.5.bias"]
+                  f"but try to load pre-trained layer with logits: {pretrain_logits}\nDropping last layer.")
+            if kwargs["head_type"] == "mlp":
+                del state_dict["classifier.5.weight"]
+                del state_dict["classifier.5.bias"]
+            else:
+                state_dict = {k: v for k, v in state_dict.items() if not k.startswith("classifier")}
         try:
             model.load_state_dict(state_dict)
         except RuntimeError as e:

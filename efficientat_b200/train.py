@@ -14,6 +14,7 @@ import torch
 from . import parallel
 from ._lib import lib
 from .helpers.utils import mixup as draw_mixup
+from .models.common import head_dropout
 
 
 def _stream():
@@ -250,7 +251,7 @@ class AudioSetTrainer:
         (loss weight, dropout rate, BatchNorm momentum / eps, DynamicConv temperatures)"""
         bn = next((m for m in self.model.modules() if isinstance(m, torch.nn.BatchNorm2d)), None)
         return (tuple(spec.shape), tuple(y.shape), teacher is not None, perm_d is not None, known is not None,
-                float(self.kd_lambda), float(self.model.classifier[4].p),
+                float(self.kd_lambda), head_dropout(self.model),
                 (float(bn.momentum), float(bn.eps)) if bn is not None else None,
                 tuple(float(getattr(m, "temperature", 0.0)) for m in self.model.modules() if hasattr(m, "temperature")))
 
@@ -311,7 +312,7 @@ class AudioSetTrainer:
     def step(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None):
         self.model.train()
         self.mel.train()
-        self.engine.dropout_p = float(self.model.classifier[4].p)     # read at call time, not at engine construction
+        self.engine.dropout_p = head_dropout(self.model)             # read at call time, not at engine construction
         with torch.cuda.device(self.flat_p.device):
             loss_acc, flat_g = self.forward_backward(wave, y, teacher, perm, lam, teacher_known)
             if self.world > 1 and self.bucketer is None:

@@ -338,6 +338,31 @@ int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, 
 int eat_act_bwd(const float* dh, const float* pre, const float* mask, int act, float* dpre, long long n,
                 cudaStream_t stream);
 
+/* ---- multi-head attention pooling classifier head (reference models/mn/attention_pooling.py:9-56, MN with
+ * head_type='multihead_attention_pooling', mn/model.py:170-172).  The projection P = m . W^T + b [B*T, 2*H*K] between
+ * the two halves below runs on the 1x1-conv GEMMs; column j of P is s*H*K + h*K + k (s = 0 attention, 1 value).
+ * Every check precedes any device call; B == 0 is a no-op. ---- */
+
+/* Frequency mean, collapse_dim(x, dim=2) at attention_pooling.py:43 (mn/utils.py:29-41): x [B,F,T,C] (dtype) ->
+ * m [B,T,C] fp32 = mean over f of xf(x); feat [B,C] fp32 (optional, overwritten) = mean over (f, t) of xf(x), the
+ * `features` output of mn/model.py:220.  xf = act(x*scale+shift) when scale is given (the last conv's BatchNorm +
+ * Hardswish, mn/model.py:160-166, in training), identity otherwise.  C a multiple of 4 (fp32) or 8 (bf16); x, m and
+ * feat 16-byte aligned. */
+int eat_freq_pool(const void* x, int dtype, const float* scale, const float* shift, int act, float* m, float* feat, int B,
+                  int F, int T, int C, cudaStream_t stream);
+/* Backward of the frequency mean: dx[b,f,t,c] = dm[b,t,c] * mul for every f (mul = 1/F), dx in the storage dtype. */
+int eat_freq_pool_bwd(const float* dm, float mul, void* dx, int dtype, int B, int F, int T, int C, cudaStream_t stream);
+/* attention_pooling.py:45-55: a = clamp(sigmoid(P_att), eps, 1-eps), v = P_val,
+ * out[b,k] = sum_h hw[h] * sum_t a v / sum_t a  (out [B,K] overwritten).  sa, r [B,H,K] (optional together, saved for
+ * backward): sa = sum_t a, r = sum_t a v / sa.  T, H, K >= 1, 0 < eps < 0.5. */
+int eat_att_pool_fwd(const float* P, const float* hw, float eps, float* out, float* sa, float* r, int B, int T, int H, int K,
+                     cudaStream_t stream);
+/* Its backward from dout [B,K]: dP [B*T, 2*H*K] overwritten (may alias P) with dP_val = dout hw a / sa and
+ * dP_att = dout hw (v - r) / sa * sigmoid'(P_att), zero where the clamp is active (torch.clamp's gradient);
+ * dhw [H] += sum_{b,k} dout r; dbias [2*H*K] += sum over rows of dP (the projection's bias gradient). */
+int eat_att_pool_bwd(const float* dout, const float* P, float* dP, const float* hw, const float* sa, const float* r, float eps,
+                     float* dhw, float* dbias, int B, int T, int H, int K, cudaStream_t stream);
+
 /* ---- training step around the network (ex_audioset.py:135-199) ---- */
 
 /* Spectrogram mixup, ex_audioset.py:145-146: out[b] = x[b]*lam[b] + x[perm[b]]*(1-lam[b]). */
