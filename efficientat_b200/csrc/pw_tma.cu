@@ -14,23 +14,27 @@
 //                           replaced IN PLACE by 32 bf16 "hi" values (64 bytes) followed by 32 bf16 "lo" values with
 //                           hi + lo = v to ~2^-17 -- the row is then a 64-element bf16 K-major row of the same
 //                           128-byte-swizzled tile the TMA wrote, which wgmma reads as is.  No second buffer.
-//   warps 4-11 consumers  : two warpgroups, one per 64-row half of the 128-row tile.  Each issues
-//                           wgmma.m64nNk16 (bf16, N = 32-column pieces of the tile) for the three products
-//                           hi*hi + lo*hi + hi*lo (fp32-grade, ~2^-16) -- the A / B descriptors simply point at the hi
-//                           or lo half of the row -- into register accumulators, one MMA group kept in flight while
-//                           the next stage is waited for.  The tile width (32, 64 or 128 columns) is a template
-//                           parameter, so every MMA is issued unconditionally.  The residual: R tiles ride the same
+//   warps 4-11 consumers  : two warpgroups, one per 64-row half of the 128-row tile.  Each issues ONE
+//                           wgmma.m64nBNk16 (bf16, BN = the whole N tile) per product and K=16 step for the three
+//                           products hi*hi + lo*hi + hi*lo (fp32-grade, ~2^-16) -- the A / B descriptors simply point at
+//                           the hi or lo half of the row -- into register accumulators, one MMA group kept in flight
+//                           while the next stage is waited for.  The tile width (any multiple of 8 up to 128 columns,
+//                           planned from N so that no tile is padded by more than 7 columns) is a template parameter,
+//                           so every MMA is issued unconditionally and reads the A slab once.  The residual: R tiles ride the same
 //                           pipeline as extra k-blocks, get the same in-place hi/lo split, and hi + lo is added to the
 //                           accumulator fragments straight from shared memory.
 //                           Epilogue from registers: shift + activation -> 128B-swizzled 16-row staging tile per warp
-//                           -> cp.async.bulk.tensor store (ragged edges clipped by the TMA unit).  BatchNorm batch
+//                           -> cp.async.bulk.tensor store (ragged edges clipped by the TMA unit); the 8 / 16 / 24-column
+//                           tail chunk of a tile goes through a tensor map of that box width, so that no store reaches
+//                           into the neighbouring N tile.  BatchNorm batch
 //                           statistics: each lane sums one column of the staged tile and keeps its partial sums in
 //                           registers across all tiles of the CTA.
 // The folded-BatchNorm scale of the epilogue is applied to the WEIGHT rows during their fix-up (W is tiny), which is
 // what lets the residual go through the accumulator unscaled.  Weights whose hi/lo tiles fit stay resident in shared
 // memory for the whole N tile; larger K streams W k-blocks with A.
 // HBM-bound at mn10 widths: algorithmic bytes per launch = 4*(M*K + M*N (+ M*N residual) + N*K).
-#include <cstdlib>
+#include <type_traits>
+#include <utility>
 
 #include "tma_common.cuh"
 
@@ -48,7 +52,7 @@ constexpr int STG_BYTES = 16 * 128;     // one staged 16 x 32 fp32 sub-tile
 struct TmaParams {
   int M, N, K;
   int BN, n_tiles, m_tiles, k_blocks, r_blocks;   // r_blocks: residual k-blocks per tile (0: no residual)
-  int bnp;                                        // BN rounded up to 128: stride of the per-column shared-memory tables
+  int bnp;                                        // BN_MAX: stride of the per-column shared-memory tables
   int stages, wres;                               // wres != 0: weight hi/lo tiles resident per N tile
   int stg_bufs;                                   // staging buffers per consumer warp (1 or 2)
   int wpre;                                       // weights arrive pre-split (bf16 hi|lo rows, scale folded): no weight fix-up
@@ -62,20 +66,17 @@ struct TmaParams {
   double* stat_sum; double* stat_sq;
 };
 
-// d[piece] += A(64 x 16) . B(32 rows x 16)^T for the NP 32-column pieces of the tile (K-major operands)
-template <int NP>
-__device__ __forceinline__ void mma_pieces(float (&d)[NP][16], uint64_t da, uint64_t db) {
-#pragma unroll
-  for (int pc = 0; pc < NP; ++pc) wgmma_n32<0, 0>(d[pc], da, db + (uint64_t)(pc * 256));   // 32 rows x 128 B = 4 KB apart
-}
-
 // EPI : 0 raw output (+ statistics), 1 + shift, 2 + shift + ReLU, 3 + shift + Hardswish   (scale lives in W)
 // XACT: -1 raw operand (gate still possible), 0 affine, 1 affine + ReLU, 2 affine + Hardswish on load
-// NP  : 32-column pieces of the N tile (BN = 32 NP)
-template <int EPI, int XACT, int NP>
+// BN  : columns of the N tile, a multiple of 8; the epilogue walks it in 32-column chunks, the last one TAIL wide
+// mapCt: output map with a TAIL-column box (unswizzled) for the last chunk of a tile that has another tile after it
+template <int EPI, int XACT, int BN>
 __global__ void __launch_bounds__(kThreads, 1)   // 13 warps: 4 on one scheduler, so at most 128 registers per thread
 pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW,
-              const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapR, const TmaParams p) {
+              const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapCt,
+              const __grid_constant__ CUtensorMap mapR, const TmaParams p) {
+  constexpr int NC = (BN + 31) / 32;                     // 32-column chunks of the epilogue
+  constexpr int TAIL = BN % 32;                          // width of the last chunk when it is not a full one
   extern __shared__ __align__(1024) unsigned char smem[];
   unsigned char* s_w = smem + p.off_w;                   // resident weights: [k_blocks][hi | lo][BN rows x 128 B]
   unsigned char* s_stg = smem + p.off_stg;               // [8 consumer warps][stg_bufs][2 KB]
@@ -97,6 +98,7 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapA)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapW)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapC)) : "memory");
+    if (TAIL != 0) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&mapCt)) : "memory");
   }
   // one-time tables: in-transform vectors (zero beyond K: act(0) = 0)
   if (XACT >= 0) {
@@ -110,13 +112,16 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
   __syncthreads();
 
   const int total_tiles = p.m_tiles * p.n_tiles;
-  constexpr int BN = 32 * NP;
   const int kb_total = p.k_blocks + p.r_blocks;          // pipeline slots per tile
   const uint32_t w_tile = (uint32_t)BN * 128u;           // bytes of one [BN x 32] weight tile
   const uint32_t stage_base = smem_u32(smem);
-  // tile walk without divisions (m fastest: a CTA stays on one N tile while it can)
-  int nt = blockIdx.x / p.m_tiles, mt = blockIdx.x - nt * p.m_tiles;
-  auto next_tile = [&]() { mt += gridDim.x; while (mt >= p.m_tiles) { mt -= p.m_tiles; ++nt; } };
+  // tile walk: the grid is a multiple of n_tiles; CTA b keeps N tile b % n_tiles (its weights stay resident) and takes every
+  // cpn-th M tile from b / n_tiles on.  The n_tiles CTAs of one M tile run at about the same time, so its A rows come from
+  // HBM once and from L2 for the other N tiles.  A CTA gets as many tiles as t = b, b + gridDim.x, ... < total_tiles counts.
+  const int cpn = gridDim.x / p.n_tiles;
+  const int nt = blockIdx.x % p.n_tiles;
+  int mt = blockIdx.x / p.n_tiles;
+  auto next_tile = [&]() { mt += cpn; };
   // (sample, M tile inside the sample) of M tile `m`; one sample = no division on the ordinary path
   auto split_tile = [&](int m, int& bs, int& jt) { if (p.n_samples == 1) { bs = 0; jt = m; } else { bs = m / p.tps; jt = m - bs * p.tps; } };
 
@@ -221,15 +226,15 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
     const uint64_t desc0 = gmma_desc(0);                      // descriptor of address 0: add (address >> 4)
     const uint64_t wres0 = desc0 + (smem_u32(s_w) >> 4);
     const uint32_t w_tile16 = w_tile >> 4;
-    float csum[NP], csq[NP];
+    float csum[NC], csq[NC];
 #pragma unroll
-    for (int c = 0; c < NP; ++c) { csum[c] = 0.f; csq[c] = 0.f; }
+    for (int c = 0; c < NC; ++c) { csum[c] = 0.f; csq[c] = 0.f; }
     int cur_nt = -1, cb = 0, s = 0;
     uint32_t ph = 0;
     auto flush_stats = [&](int nt_old) {
-      // lane partials -> shared, combine the eight warps, one fp64 atomic per channel
+      // lane partials -> shared, combine the eight warps, one fp64 atomic per channel (lanes past a tail chunk hold 0)
 #pragma unroll
-      for (int c = 0; c < NP; ++c) { my_stat[c * 32 + lane] = csum[c]; my_stat[bnp + c * 32 + lane] = csq[c]; csum[c] = 0.f; csq[c] = 0.f; }
+      for (int c = 0; c < NC; ++c) { my_stat[c * 32 + lane] = csum[c]; my_stat[bnp + c * 32 + lane] = csq[c]; csum[c] = 0.f; csq[c] = 0.f; }
       asm volatile("bar.sync 1, 256;" ::: "memory");
       for (int e = ctid; e < BN; e += kConsThreads) {
         const int n = nt_old * BN + e;
@@ -254,11 +259,10 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         cur_nt = nt;
       }
       next_tile();
-      float acc[NP][16];
+      // m64nBN fragment: acc[16 c + 4 j + ...] holds columns 32 c + 8 j + fc (+1) of chunk c
+      float acc[BN / 2];
 #pragma unroll
-      for (int c = 0; c < NP; ++c)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[c][i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       // the group of MMAs on stage `pend` may still be running; a stage is released once its group has completed
       int pend = -1;
       auto release = [&](int st) {
@@ -279,9 +283,9 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
             const uint64_t ko = (uint64_t)(j * 2);                // 16 bf16 = 32 bytes along K, in 16-byte units
-            mma_pieces<NP>(acc, a_hi + ko, w_hi + ko);
-            mma_pieces<NP>(acc, a_lo + ko, w_hi + ko);
-            mma_pieces<NP>(acc, a_hi + ko, w_lo + ko);
+            wgmma_kk<BN>(acc, a_hi + ko, w_hi + ko);
+            wgmma_kk<BN>(acc, a_lo + ko, w_hi + ko);
+            wgmma_kk<BN>(acc, a_hi + ko, w_lo + ko);
           }
           wgmma_commit();
           wgmma_wait<1>();                                       // the previous stage's group has completed
@@ -291,26 +295,27 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
           // residual block jr: D[:, 32 jr .. 32 jr + 31] += R_hi + R_lo, read from the split tile (row r: hi of column c
           // in chunk c / 8, lo in chunk 4 + c / 8, element c % 8)
           wgmma_wait<0>();
-#pragma unroll
-          for (int c = 0; c < NP; ++c) wgmma_fence_regs(acc[c]);
+          wgmma_fence_regs(acc);
           if (pend >= 0) { release(pend); pend = -1; }
           const int jr = kb - p.k_blocks;
           const unsigned char* tile = smem + (size_t)s * p.stage_bytes;
           const int r0 = g * 64 + wq * 16 + fr;
 #pragma unroll
-          for (int c = 0; c < NP; ++c) {
+          for (int c = 0; c < NC; ++c) {
             if (c == jr) {
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
+                if (32 * c + 8 * j < BN) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  const int r = r0 + 8 * h;
-                  const uint32_t e = (uint32_t)fc * 2;
-                  const __nv_bfloat162 hi = *reinterpret_cast<const __nv_bfloat162*>(tile + swz(r, j) + e);
-                  const __nv_bfloat162 lo = *reinterpret_cast<const __nv_bfloat162*>(tile + swz(r, 4 + j) + e);
-                  const float2 fh = __bfloat1622float2(hi), fl = __bfloat1622float2(lo);
-                  acc[c][4 * j + 2 * h] += fh.x + fl.x;
-                  acc[c][4 * j + 2 * h + 1] += fh.y + fl.y;
+                  for (int h = 0; h < 2; ++h) {
+                    const int r = r0 + 8 * h;
+                    const uint32_t e = (uint32_t)fc * 2;
+                    const __nv_bfloat162 hi = *reinterpret_cast<const __nv_bfloat162*>(tile + swz(r, j) + e);
+                    const __nv_bfloat162 lo = *reinterpret_cast<const __nv_bfloat162*>(tile + swz(r, 4 + j) + e);
+                    const float2 fh = __bfloat1622float2(hi), fl = __bfloat1622float2(lo);
+                    acc[16 * c + 4 * j + 2 * h] += fh.x + fl.x;
+                    acc[16 * c + 4 * j + 2 * h + 1] += fh.y + fl.y;
+                  }
                 }
               }
             }
@@ -323,14 +328,17 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
         wgmma_wait<0>();
         release(pend);
       }
-#pragma unroll
-      for (int c = 0; c < NP; ++c) wgmma_fence_regs(acc[c]);
-      // ---- epilogue: fragment -> shift + activation -> swizzled 16 x 32 staging tile -> TMA store
+      wgmma_fence_regs(acc);
+      // ---- epilogue: fragment -> shift + activation -> staging tile -> TMA store.  A chunk is staged as a swizzled
+      // 16 x 32 tile and stored through mapC, which clips at N.  A tail chunk (cw < 32 columns) with another N tile after
+      // it is staged as plain 16 x cw rows and stored through mapCt instead.
       const int row0 = m0 + g * 64 + wq * 16;
       const int rows_left = min(16, p.tile_rps - row0);        // <= 0: nothing of this warp's slab is inside the sample
 #pragma unroll
-      for (int c = 0; c < NP; ++c) {
-        if (c * 32 < BN && n0 + c * 32 < p.N) {
+      for (int c = 0; c < NC; ++c) {
+        const int cw = (TAIL != 0 && c == NC - 1) ? TAIL : 32;
+        const bool tail = cw < 32 && n0 + BN < p.N;
+        if (n0 + c * 32 < p.N) {
           unsigned char* buf = stg + (size_t)cb * STG_BYTES;
           // the store issued from this buffer (two chunks ago, or the previous one with a single buffer) has drained
           if (p.stg_bufs == 2) { cb ^= 1; if (lane == 0) tma_wait_read<1>(); }
@@ -338,31 +346,42 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
           __syncwarp();
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const int cc = 8 * j + fc;
-            float2 v0 = make_float2(acc[c][4 * j], acc[c][4 * j + 1]), v1 = make_float2(acc[c][4 * j + 2], acc[c][4 * j + 3]);
-            if (EPI != 0) {
-              const float2 sh = *reinterpret_cast<const float2*>(s_shift + c * 32 + cc);
-              v0.x = act_out<EPI>(v0.x + sh.x); v0.y = act_out<EPI>(v0.y + sh.y);
-              v1.x = act_out<EPI>(v1.x + sh.x); v1.y = act_out<EPI>(v1.y + sh.y);
+            if (32 * c + 8 * j < BN) {
+              const int cc = 8 * j + fc;
+              const float* a4 = acc + 16 * c + 4 * j;
+              float2 v0 = make_float2(a4[0], a4[1]), v1 = make_float2(a4[2], a4[3]);
+              if (EPI != 0) {
+                const float2 sh = *reinterpret_cast<const float2*>(s_shift + c * 32 + cc);
+                v0.x = act_out<EPI>(v0.x + sh.x); v0.y = act_out<EPI>(v0.y + sh.y);
+                v1.x = act_out<EPI>(v1.x + sh.x); v1.y = act_out<EPI>(v1.y + sh.y);
+              }
+              if (tail) {
+                *reinterpret_cast<float2*>(buf + (fr * cw + cc) * 4) = v0;
+                *reinterpret_cast<float2*>(buf + ((fr + 8) * cw + cc) * 4) = v1;
+              } else {
+                const uint32_t co = (uint32_t)(((cc >> 2) << 4) + (cc & 3) * 4);
+                *reinterpret_cast<float2*>(buf + fr * 128 + (co ^ ((fr & 7) << 4))) = v0;
+                *reinterpret_cast<float2*>(buf + (fr + 8) * 128 + (co ^ (((fr + 8) & 7) << 4))) = v1;
+              }
             }
-            const uint32_t co = (uint32_t)(((cc >> 2) << 4) + (cc & 3) * 4);
-            *reinterpret_cast<float2*>(buf + fr * 128 + (co ^ ((fr & 7) << 4))) = v0;
-            *reinterpret_cast<float2*>(buf + (fr + 8) * 128 + (co ^ (((fr + 8) & 7) << 4))) = v1;
           }
           if (do_stats) {
             __syncwarp();
             // lane = column: sum the staged column over the rows of this slab that lie inside M
             float s1 = 0.f, s2 = 0.f;
             const int cj = lane >> 2, ci = lane & 3;
-            for (int r = 0; r < rows_left; ++r) {
-              const float x = *reinterpret_cast<const float*>(buf + r * 128 + ((cj ^ (r & 7)) << 4) + ci * 4);
-              s1 += x; s2 = fmaf(x, x, s2);
+            if (lane < cw) {
+              for (int r = 0; r < rows_left; ++r) {
+                const uint32_t o = tail ? (uint32_t)(r * cw + lane) * 4 : (uint32_t)(r * 128 + ((cj ^ (r & 7)) << 4) + ci * 4);
+                const float x = *reinterpret_cast<const float*>(buf + o);
+                s1 += x; s2 = fmaf(x, x, s2);
+              }
             }
             csum[c] += s1; csq[c] += s2;
           }
           fence_proxy_async();
           __syncwarp();
-          if (lane == 0 && rows_left > 0) { tma_store_3d(&mapC, smem_u32(buf), n0 + c * 32, row0, bs); tma_commit(); }
+          if (lane == 0 && rows_left > 0) { tma_store_3d(tail ? &mapCt : &mapC, smem_u32(buf), n0 + c * 32, row0, bs); tma_commit(); }
         }
       }
     }
@@ -452,42 +471,75 @@ int make_map_bf16(CUtensorMap* map, const void* ptr, long long rows, long long c
   return EAT_OK;
 }
 
+// [samples, rows, cols] fp32 output viewed through a {cw columns, 16 rows, 1} box without swizzle (cw = 8, 16 or 24): the
+// store of a tile's tail chunk, which must not write the columns of the next N tile
+int make_map_tail(CUtensorMap* map, const void* ptr, long long samples, long long rows, long long cols, int cw) {
+  EncodeTiledFn enc = encode_fn();
+  if (enc == nullptr) { eat_set_error("pw_tma: cuTensorMapEncodeTiled is not available from this driver"); return EAT_ERR_CUDA; }
+  cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)samples};
+  cuuint64_t gstride[2] = {(cuuint64_t)cols * 4, (cuuint64_t)(rows * cols * 4)};
+  cuuint32_t box[3] = {(cuuint32_t)cw, 16, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { eat_set_error("pw_tma: cuTensorMapEncodeTiled (tail store) failed"); return EAT_ERR_CUDA; }
+  return EAT_OK;
+}
+
 constexpr size_t kSmemLimit = 227 * 1024;
 
-template <int EPI, int XACT, int NP>
-int launch_kernel(const CUtensorMap& mA, const CUtensorMap& mW, const CUtensorMap& mC, const CUtensorMap& mR, const TmaParams& p,
-                  size_t smem, int tiles, cudaStream_t st) {
+struct Maps { CUtensorMap A, W, C, Ct, R; };
+
+template <int EPI, int XACT, int BN>
+int launch_kernel(const Maps& m, const TmaParams& p, size_t smem, int tiles, cudaStream_t st) {
   static unsigned long long attr_mask = 0;
-  if (int rc = eat_opt_in_smem(pw_tma_kernel<EPI, XACT, NP>, kSmemLimit, attr_mask)) return rc;
+  if (int rc = eat_opt_in_smem(pw_tma_kernel<EPI, XACT, BN>, kSmemLimit, attr_mask)) return rc;
   int dev = 0, sms = kNumSMs;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  pw_tma_kernel<EPI, XACT, NP><<<tiles < sms ? tiles : sms, kThreads, smem, st>>>(mA, mW, mC, mR, p);
+  // persistent grid, a multiple of n_tiles (the kernel's tile walk); tiles is one as well
+  const int grid = min(tiles, max(p.n_tiles, sms / p.n_tiles * p.n_tiles));
+  pw_tma_kernel<EPI, XACT, BN><<<grid, kThreads, smem, st>>>(m.A, m.W, m.C, m.Ct, m.R, p);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
+}
+
+// Tile widths with a compiled kernel.  The raw-output variant (training forward with batch statistics, every data
+// gradient) has one at every multiple of 8; the epilogue variants (inference) keep 32 / 64 / 128.
+template <int EPI>
+using Widths = std::conditional_t<EPI == 0,
+                                  std::integer_sequence<int, 8, 16, 24, 32, 40, 48, 56, 64, 72, 80, 88, 96, 104, 112, 120, 128>,
+                                  std::integer_sequence<int, 32, 64, 128>>;
+
+// narrowest compiled width >= bn
+template <int... W>
+constexpr int fit_width(std::integer_sequence<int, W...>, int bn) {
+  int best = BN_MAX;
+  for (int w : {W...}) if (w >= bn && w < best) best = w;
+  return best;
+}
+
+template <int EPI, int XACT, int... W>
+int launch_width(std::integer_sequence<int, W...>, const Maps& m, const TmaParams& p, size_t smem, int tiles, cudaStream_t st) {
+  int rc = EAT_ERR_UNSUPPORTED;
+  const bool found = ((p.BN == W && (rc = launch_kernel<EPI, XACT, W>(m, p, smem, tiles, st), true)) || ...);
+  if (!found) eat_set_error("pw_tma: no kernel for this tile width");
+  return rc;
 }
 
 struct WeightWs { int trans; void* ws; size_t bytes; const float* att; int dyn_k; };   // att != nullptr: DynamicConv kernel mix
 
 template <int EPI, int XACT>
 int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams p, cudaStream_t st, WeightWs ws) {
-  // ---- tiling.  Shared-memory traffic per k-block of one M tile is n_tiles * (TMA write 16 KB + fix-up 32 KB + 24 KB of A
-  // operand reads) + 320 B per padded output column: wide N tiles amortise the A side.  The widest tile is bounded by the
-  // consumer registers (a 64 x 128 fp32 accumulator per warpgroup = 64 registers per thread).
-  // Tile widths are 32, 64 or 128 columns (compile-time piece counts: every MMA is issued unconditionally).
-  int bn_max = BN_MAX;
-  if (const char* e = getenv("EAT_TMA_BNMAX")) { const int v = atoi(e); if (v == 64 || v == BN_MAX) bn_max = v; }
-  if (p.N <= bn_max) { p.BN = p.N <= 32 ? 32 : (p.N <= 64 ? 64 : 128); p.n_tiles = 1; }
-  else {                                   // several N tiles
-    int best = 0; long long best_cost = 0;
-    for (int bn = 64; bn <= bn_max; bn *= 2) {
-      const long long nt = ceil_div(p.N, bn);
-      const long long cost = nt * 72 * 1024 + nt * bn * 320;
-      if (best == 0 || cost < best_cost || (cost == best_cost && bn > best)) { best = bn; best_cost = cost; }
-    }
-    p.BN = best; p.n_tiles = ceil_div(p.N, best);
-  }
-  p.bnp = 128;
+  // ---- tiling.  Every N tile lands and fixes up the A tile again (TMA write 16 KB + fix-up 32 KB per k-block), so N is
+  // cut into as few tiles as the consumer registers allow (a 64 x 128 fp32 accumulator per warpgroup = 64 registers per
+  // thread), of equal width rounded up to 8 columns: tensor-core work is padded by at most 7 columns per tile.  A width
+  // without a compiled kernel runs on the next wider one (the TMA unit zero-fills the weight rows past N).
+  p.n_tiles = ceil_div(p.N, BN_MAX);
+  p.BN = fit_width(Widths<EPI>{}, (ceil_div(p.N, p.n_tiles) + 7) & ~7);
+  p.n_tiles = ceil_div(p.N, p.BN);
+  p.bnp = BN_MAX;
   if (p.n_samples < 1) { p.n_samples = 1; p.tile_rps = p.M; }
   p.tps = ceil_div(p.tile_rps, BM);
   p.m_tiles = p.n_samples * p.tps;
@@ -518,7 +570,8 @@ int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams 
   const size_t smem = off;
   if (smem > kSmemLimit) { eat_set_error("pw_tma: shared-memory carve-up exceeds its budget"); return EAT_ERR_UNSUPPORTED; }
   // ---- tensor maps
-  CUtensorMap mA, mW, mC, mR;
+  Maps m;
+  CUtensorMap &mA = m.A, &mW = m.W, &mC = m.C, &mR = m.R;
   const long long ns = p.n_samples, rps = p.tile_rps;
   if (int rc = make_map3(&mA, A, ns, rps, p.K, BM, 4)) return rc;
   p.wpre = 0;
@@ -546,11 +599,13 @@ int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams 
     if (int rc = make_map3(&mW, W, 1, p.N, p.K, p.BN, 4)) return rc;
   }
   if (int rc = make_map3(&mC, C, ns, rps, p.N, 16, 4)) return rc;
+  if (p.n_tiles > 1 && p.BN % 32 != 0) {
+    if (int rc = make_map_tail(&m.Ct, C, ns, rps, p.N, p.BN % 32)) return rc;
+  } else {
+    m.Ct = mC;                                               // unused: every chunk is a full one
+  }
   if (int rc = make_map3(&mR, R != nullptr ? R : C, ns, rps, p.N, BM, 4)) return rc;
-  const int tiles = p.m_tiles * p.n_tiles;
-  if (p.BN == 32) return launch_kernel<EPI, XACT, 1>(mA, mW, mC, mR, p, smem, tiles, st);
-  if (p.BN == 64) return launch_kernel<EPI, XACT, 2>(mA, mW, mC, mR, p, smem, tiles, st);
-  return launch_kernel<EPI, XACT, 4>(mA, mW, mC, mR, p, smem, tiles, st);
+  return launch_width<EPI, XACT>(Widths<EPI>{}, m, p, smem, p.m_tiles * p.n_tiles, st);
 }
 
 template <int EPI>

@@ -78,6 +78,56 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
       : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
 
+// m64nNk16 for any N = 8, 16, ..., 128, both operands K-major: d[N / 2] is the fragment above with j = 0 .. N / 8 - 1.
+// EAT_WG_S<N> / EAT_WG_O<N> spell out the N / 2 accumulator placeholders and operands; the descriptors and the scale-d
+// flag follow them as operands N / 2 .. N / 2 + 2.
+#define EAT_WG_S8 "%0, %1, %2, %3"
+#define EAT_WG_S16 EAT_WG_S8 ", %4, %5, %6, %7"
+#define EAT_WG_S24 EAT_WG_S16 ", %8, %9, %10, %11"
+#define EAT_WG_S32 EAT_WG_S24 ", %12, %13, %14, %15"
+#define EAT_WG_S40 EAT_WG_S32 ", %16, %17, %18, %19"
+#define EAT_WG_S48 EAT_WG_S40 ", %20, %21, %22, %23"
+#define EAT_WG_S56 EAT_WG_S48 ", %24, %25, %26, %27"
+#define EAT_WG_S64 EAT_WG_S56 ", %28, %29, %30, %31"
+#define EAT_WG_S72 EAT_WG_S64 ", %32, %33, %34, %35"
+#define EAT_WG_S80 EAT_WG_S72 ", %36, %37, %38, %39"
+#define EAT_WG_S88 EAT_WG_S80 ", %40, %41, %42, %43"
+#define EAT_WG_S96 EAT_WG_S88 ", %44, %45, %46, %47"
+#define EAT_WG_S104 EAT_WG_S96 ", %48, %49, %50, %51"
+#define EAT_WG_S112 EAT_WG_S104 ", %52, %53, %54, %55"
+#define EAT_WG_S120 EAT_WG_S112 ", %56, %57, %58, %59"
+#define EAT_WG_S128 EAT_WG_S120 ", %60, %61, %62, %63"
+#define EAT_WG_O8 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+#define EAT_WG_O16 EAT_WG_O8, "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+#define EAT_WG_O24 EAT_WG_O16, "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+#define EAT_WG_O32 EAT_WG_O24, "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+#define EAT_WG_O40 EAT_WG_O32, "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+#define EAT_WG_O48 EAT_WG_O40, "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+#define EAT_WG_O56 EAT_WG_O48, "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
+#define EAT_WG_O64 EAT_WG_O56, "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define EAT_WG_O72 EAT_WG_O64, "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+#define EAT_WG_O80 EAT_WG_O72, "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+#define EAT_WG_O88 EAT_WG_O80, "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43])
+#define EAT_WG_O96 EAT_WG_O88, "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+#define EAT_WG_O104 EAT_WG_O96, "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+#define EAT_WG_O112 EAT_WG_O104, "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+#define EAT_WG_O120 EAT_WG_O112, "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59])
+#define EAT_WG_O128 EAT_WG_O120, "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+#define EAT_WG_CASE(W, DA, DB, ONE)                                                                                     \
+  if constexpr (N == W)                                                                                                 \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #ONE ", 0;\n"                                                     \
+                 "wgmma.mma_async.sync.aligned.m64n" #W "k16.f32.bf16.bf16 {" EAT_WG_S##W "}, %" #DA ", %" #DB ", p, 1, 1, 0, 0;\n}\n" \
+                 : EAT_WG_O##W : "l"(da), "l"(db), "r"(1));
+template <int N>
+__device__ __forceinline__ void wgmma_kk(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N % 8 == 0 && N >= 8 && N <= 128, "m64nNk16: N is a multiple of 8 up to 128 here");
+  EAT_WG_CASE(8, 4, 5, 6) EAT_WG_CASE(16, 8, 9, 10) EAT_WG_CASE(24, 12, 13, 14) EAT_WG_CASE(32, 16, 17, 18)
+  EAT_WG_CASE(40, 20, 21, 22) EAT_WG_CASE(48, 24, 25, 26) EAT_WG_CASE(56, 28, 29, 30) EAT_WG_CASE(64, 32, 33, 34)
+  EAT_WG_CASE(72, 36, 37, 38) EAT_WG_CASE(80, 40, 41, 42) EAT_WG_CASE(88, 44, 45, 46) EAT_WG_CASE(96, 48, 49, 50)
+  EAT_WG_CASE(104, 52, 53, 54) EAT_WG_CASE(112, 56, 57, 58) EAT_WG_CASE(120, 60, 61, 62) EAT_WG_CASE(128, 64, 65, 66)
+}
+#undef EAT_WG_CASE
+
 __device__ __forceinline__ uint32_t swz(int row, int chunk) {   // byte offset of a 16-byte chunk in a [rows][128 B] tile
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((chunk ^ (row & 7)) << 4));
 }
