@@ -42,10 +42,11 @@ __device__ __forceinline__ float act_fwd(float v, int act) {
   return v;
 }
 // derivative of the activation w.r.t. its input, evaluated at pre-activation v
-// (torch: hardswish' = 0 for v<-3, 1 for v>3, (2v+3)/6 otherwise; relu' = v>0)
+// (hardswish' = 0 for v<=-3, 1 for v>=3, (2v+3)/6 in between, as torch 2.x's hardswish_backward -- the torch the golden
+// vectors and the oracle are produced with; torch 1.13 gave -1/2 at -3 and 3/2 at 3; relu' = v>0)
 __device__ __forceinline__ float act_bwd(float v, int act) {
   if (act == EAT_ACT_RELU) return v > 0.f ? 1.f : 0.f;
-  if (act == EAT_ACT_HSWISH) return v < -3.f ? 0.f : (v <= 3.f ? (2.f * v + 3.f) * (1.f / 6.f) : 1.f);
+  if (act == EAT_ACT_HSWISH) return v <= -3.f ? 0.f : (v < 3.f ? (2.f * v + 3.f) * (1.f / 6.f) : 1.f);
   return 1.f;
 }
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + expf(-v)); }

@@ -39,17 +39,6 @@ template <> struct Vec4IO<__nv_bfloat16> {
 };
 
 // ------------------------------------------------------------------------------------------
-// Block-level reduction of per-thread channel partial sums.
-// Thread layout: cvi = tid % cv (channel vector), slot = tid / cv.  s_acc has C floats (x2 if sq).
-template <int V>
-__device__ __forceinline__ void block_channel_reduce(float (&sum)[V], float* s_acc, int C, int cvi, bool active) {
-  if (active) {
-#pragma unroll
-    for (int i = 0; i < V; ++i) atomicAdd(&s_acc[cvi * V + i], sum[i]);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
 // Stem: x [B, F, T] fp32 (one input channel) -> out [B, Fo, To, C] ; 3x3, pad 1, stride s.
 template <typename TO>
 __global__ void __launch_bounds__(kThreads) stem_kernel(
@@ -60,19 +49,16 @@ __global__ void __launch_bounds__(kThreads) stem_kernel(
   constexpr int V = Vec<TO>::N;
   extern __shared__ float smem[];
   float* s_w = smem;            // [9][C]
-  float* s_sum = s_w + 9 * C;   // [C]
-  float* s_sq = s_sum + C;      // [C]
   for (int i = threadIdx.x; i < 9 * C; i += kThreads) { int c = i % C, tap = i / C; s_w[i] = w[c * 9 + tap]; }
-  for (int i = threadIdx.x; i < 2 * C; i += kThreads) s_sum[i] = 0.f;
   __syncthreads();
   const int cv = C / V;
   const int ppb = kThreads / cv;
   const int cvi = threadIdx.x % cv, slot = threadIdx.x / cv;
   const bool active = slot < ppb;
   const long long npix = (long long)B * Fo * To;
-  float lsum[V], lsq[V];
+  double lsum[V], lsq[V];      // fp64 from the first term: in fp32, E[x^2] - E[x]^2 cancels when |mean| >> std
 #pragma unroll
-  for (int i = 0; i < V; ++i) { lsum[i] = 0.f; lsq[i] = 0.f; }
+  for (int i = 0; i < V; ++i) { lsum[i] = 0.0; lsq[i] = 0.0; }
   if (active) {
     // 32-bit index math (the launcher guarantees npix < 2^31): three 64-bit div/mod per pixel cost more than the 9 taps
     const unsigned ppx = (unsigned)To * (unsigned)Fo;
@@ -101,18 +87,25 @@ __global__ void __launch_bounds__(kThreads) stem_kernel(
         for (int i = 0; i < V; ++i) acc[i] = act_fwd(fmaf(acc[i], scale[cvi * V + i], shift[cvi * V + i]), act);
       } else {
 #pragma unroll
-        for (int i = 0; i < V; ++i) { lsum[i] += acc[i]; lsq[i] = fmaf(acc[i], acc[i], lsq[i]); }
+        for (int i = 0; i < V; ++i) { lsum[i] += acc[i]; lsq[i] = fma((double)acc[i], (double)acc[i], lsq[i]); }
       }
       Vec<TO>::store(out + (size_t)pix * C + cvi * V, acc);
     }
   }
   if (stat_sum != nullptr) {
-    block_channel_reduce<V>(lsum, s_sum, C, cvi, active);
-    block_channel_reduce<V>(lsq, s_sq, C, cvi, active);
+    // the weight table is no longer read: its space holds the CTA's fp64 sums ([2][C] doubles <= [9][C] floats)
+    double* d_sum = reinterpret_cast<double*>(smem);
+    __syncthreads();
+    for (int i = threadIdx.x; i < 2 * C; i += kThreads) d_sum[i] = 0.0;
+    __syncthreads();
+    if (active) {
+#pragma unroll
+      for (int i = 0; i < V; ++i) { atomicAdd(&d_sum[cvi * V + i], lsum[i]); atomicAdd(&d_sum[C + cvi * V + i], lsq[i]); }
+    }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += kThreads) {
-      atomicAdd(stat_sum + c, (double)s_sum[c]);
-      atomicAdd(stat_sq + c, (double)s_sq[c]);
+      atomicAdd(stat_sum + c, d_sum[c]);
+      atomicAdd(stat_sq + c, d_sum[C + c]);
     }
   }
 }
@@ -127,14 +120,15 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
     const float* __restrict__ scale, const float* __restrict__ shift, int act,
     double* __restrict__ stat_sum, double* __restrict__ stat_sq) {
   constexpr int V = 4, U = 4;
-  __shared__ float s_sum[2 * 64];
-  for (int i = threadIdx.x; i < 2 * C; i += kThreads) s_sum[i] = 0.f;
+  __shared__ double s_sum[2 * 64];
+  for (int i = threadIdx.x; i < 2 * C; i += kThreads) s_sum[i] = 0.0;
   __syncthreads();
   const int cv = C / V;
   const int ppb = kThreads / cv;
   const int cvi = threadIdx.x % cv, slot = threadIdx.x / cv;
   const bool active = slot < ppb;
-  float wr[9][V], sc[V], sh[V], lsum[V], lsq[V];
+  float wr[9][V], sc[V], sh[V];
+  double lsum[V], lsq[V];      // fp64 from the first term: in fp32, E[x^2] - E[x]^2 cancels when |mean| >> std
 #pragma unroll
   for (int q = 0; q < 9; ++q)
 #pragma unroll
@@ -143,7 +137,7 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
   for (int i = 0; i < V; ++i) {
     sc[i] = scale != nullptr ? scale[cvi * V + i] : 1.f;
     sh[i] = scale != nullptr ? shift[cvi * V + i] : 0.f;
-    lsum[i] = 0.f; lsq[i] = 0.f;
+    lsum[i] = 0.0; lsq[i] = 0.0;
   }
   const int rows = B * Fo;
   if (active) {
@@ -181,7 +175,7 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
             for (int i = 0; i < V; ++i) acc[i] = act_fwd(fmaf(acc[i], sc[i], sh[i]), act);
           } else {
 #pragma unroll
-            for (int i = 0; i < V; ++i) { lsum[i] += acc[i]; lsq[i] = fmaf(acc[i], acc[i], lsq[i]); }
+            for (int i = 0; i < V; ++i) { lsum[i] += acc[i]; lsq[i] = fma((double)acc[i], (double)acc[i], lsq[i]); }
           }
           *reinterpret_cast<float4*>(orow + (size_t)to * C) = make_float4(acc[0], acc[1], acc[2], acc[3]);
         }
@@ -195,8 +189,8 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
     }
     __syncthreads();
     for (int c = threadIdx.x; c < C; c += kThreads) {
-      atomicAdd(stat_sum + c, (double)s_sum[c]);
-      atomicAdd(stat_sq + c, (double)s_sum[C + c]);
+      atomicAdd(stat_sum + c, s_sum[c]);
+      atomicAdd(stat_sq + c, s_sum[C + c]);
     }
   }
 }
@@ -674,7 +668,7 @@ int eat_stem_fwd(const float* x, const float* w, void* out, int out_dtype, int B
     return EAT_OK;
   }
   int grid = grid_for(npix, ppb, kNumSMs * 8);
-  size_t smem = (size_t)11 * C * sizeof(float);
+  size_t smem = (size_t)9 * C * sizeof(float);
   if (out_dtype == EAT_BF16)
     stem_kernel<__nv_bfloat16><<<grid, kThreads, smem, st>>>(x, w, (__nv_bfloat16*)out, B, F, T, Fo, To, C, stride, scale, shift, act, stat_sum, stat_sq);
   else
