@@ -1,5 +1,6 @@
 """Host-side helpers the reference scripts import from helpers/utils.py (NAME_TO_WIDTH :1-32, label table :35-46, LR
-schedule :56-84, mixup :90-95).  Pure Python / numpy, re-implemented with the same semantics."""
+schedule :56-84, mixup :90-95, mixstyle :101-121).  Re-implemented with the same semantics and the same host RNG draws;
+mixstyle's arithmetic runs on the device (eat_mixstyle)."""
 import csv
 import os
 
@@ -59,3 +60,37 @@ def mixup(size, alpha):
     lambd = np.random.beta(alpha, alpha, size).astype(np.float32)
     lambd = np.maximum(lambd, 1.0 - lambd)
     return rn_indices, torch.from_numpy(lambd)
+
+
+def mixstyle(x, p=0.4, alpha=0.4, eps=1e-6, mix_labels=False):
+    """Frequency-wise MixStyle (helpers/utils.py:101-121) on a [B, 1, F, T] fp32 CUDA spectrogram, by `eat_mixstyle`.
+
+    Same host RNG draws in the same order as the reference: `np.random.rand()` for the skip test (x comes back
+    unchanged with probability 1 - p), then `Beta(alpha, alpha).sample((B, 1, 1, 1))` and `torch.randperm(B)` on the
+    CPU generators.  mix_labels=True also returns (perm, lambda) on x's device, as the reference does.  The statistics
+    are not differentiated through (the reference detaches them) and gradients w.r.t. x are not implemented."""
+    from torch.distributions.beta import Beta
+
+    from .._lib import lib
+    if np.random.rand() > p:
+        return x
+    if not x.is_cuda:
+        raise RuntimeError("mixstyle: x must be a CUDA tensor (the product path has no CPU fallback)")
+    if x.requires_grad:
+        raise NotImplementedError("mixstyle: gradients w.r.t. the input spectrogram are not implemented")
+    if x.dim() != 4 or x.shape[1] != 1 or x.dtype != torch.float32:
+        raise ValueError(f"mixstyle: expects a [B, 1, F, T] fp32 spectrogram, got {x.dtype} {tuple(x.shape)}")
+    B, _, F, T = x.shape
+    lmda = Beta(alpha, alpha).sample((B, 1, 1, 1))
+    perm = torch.randperm(B)
+    x = x.contiguous()
+    out = torch.empty_like(x)
+    stats = torch.empty(2 * B * F, device=x.device, dtype=torch.float32)
+    with torch.cuda.device(x.device):
+        perm_d = perm.to(device=x.device, dtype=torch.int32)
+        lam_d = lmda.to(device=x.device, dtype=torch.float32).reshape(B)
+        lib().mixstyle(x.data_ptr(), perm_d.data_ptr(), lam_d.data_ptr(), float(eps), stats.data_ptr(), out.data_ptr(),
+                       B, F, T, torch.cuda.current_stream().cuda_stream)
+    if mix_labels:
+        return out, perm.to(x.device), lmda.to(x.device)
+    return out

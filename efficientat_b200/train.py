@@ -229,22 +229,26 @@ class AudioSetTrainer:
 
     def _core(self, spec4, y, teacher, perm_d, lam_d, known=None):
         """model forward + loss + backward on device tensors -> (loss_acc, flat gradient arena)"""
-        L = lib()
-        B = spec4.shape[0]
         logits, _, saved = self.engine._forward_train(spec4)
-        dlogits = torch.empty_like(logits)
-        loss_acc = torch.zeros(2, device=spec4.device, dtype=torch.float64)
-        # without a teacher the label loss carries weight 1 (ex_audioset.py:182-183)
-        L.bce_kd_loss(logits.data_ptr(), y.data_ptr(), teacher.data_ptr() if teacher is not None else 0,
-                      known.data_ptr() if known is not None else 0,
-                      perm_d.data_ptr() if perm_d is not None else 0, lam_d.data_ptr() if lam_d is not None else 0,
-                      self.kd_lambda, B, logits.shape[1], dlogits.data_ptr(), loss_acc.data_ptr(), _stream())
+        loss_acc, dlogits = self._loss(logits, y, teacher, perm_d, lam_d, known)
         if self.bucketer is not None:
             grads = self.engine._backward(saved, dlogits, on_ready=self.bucketer.ready)
             self.bucketer.finish(grads[None])                     # joins the side stream: the arena is reduced (sum)
         else:
             grads = self.engine._backward(saved, dlogits)
         return loss_acc, grads[None]
+
+    def _loss(self, logits, y, teacher, perm_d, lam_d, known):
+        """-> (loss_acc, dlogits): the loss of the step and its gradient w.r.t. the logits, on the device"""
+        B = logits.shape[0]
+        dlogits = torch.empty_like(logits)
+        loss_acc = torch.zeros(2, device=logits.device, dtype=torch.float64)
+        # without a teacher the label loss carries weight 1 (ex_audioset.py:182-183)
+        lib().bce_kd_loss(logits.data_ptr(), y.data_ptr(), teacher.data_ptr() if teacher is not None else 0,
+                          known.data_ptr() if known is not None else 0,
+                          perm_d.data_ptr() if perm_d is not None else 0, lam_d.data_ptr() if lam_d is not None else 0,
+                          self.kd_lambda, B, logits.shape[1], dlogits.data_ptr(), loss_acc.data_ptr(), _stream())
+        return loss_acc, dlogits
 
     def _graph_key(self, spec, y, teacher, perm_d, known):
         """everything a captured graph bakes in: shapes, optional-operand presence and the host scalars passed by value

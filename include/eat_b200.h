@@ -380,6 +380,31 @@ int eat_bce_kd_loss(const float* logits, const float* y, const float* teacher, c
 int eat_adam_step(float* p, const float* g, float* m, float* v, long long n, float lr, float beta1, float beta2,
                   float eps, float weight_decay, int adamw, int step, float grad_scale, cudaStream_t stream);
 
+/* ---- fine-tuning step (ex_esc50.py:96-118, ex_dcase20.py:98-123, ex_openmic.py:97-121; FSD50K, ex_fsd50k.py:97-115,
+ * is eat_bce_kd_loss without a teacher).  Every check precedes any device call; B == 0 is a no-op. ---- */
+
+/* Softmax cross-entropy, F.cross_entropy(logits, y, reduction="none").mean(), and its gradient.  Exactly one of
+ * y_index (int32 [B], class indices) and y_prob (fp32 [B, C], probability rows) is given.  perm/lam (optional,
+ * together): the mixup blend lam*CE(z, y) + (1-lam)*CE(z, y[perm]) as one CE against the blended target y_mix.
+ * loss_acc[0] (fp64, caller-zeroed) += mean over b of sum_c y_mix * (lse(z_b) - z_bc);
+ * dlogits (optional) = (S * softmax(z) - y_mix) / B with S = sum_c y_mix per row.  Any C >= 1.  An index outside
+ * [0, C) makes the loss NaN. */
+int eat_ce_loss(const float* logits, const int* y_index, const float* y_prob, const int* perm, const float* lam, int B,
+                int C, float* dlogits, double* loss_acc, cudaStream_t stream);
+/* OpenMIC's masked multi-label BCE, ex_openmic.py:101-121: y [B, *] (row stride y_stride) is binarised (> 0.5) before
+ * the optional mixup blend; mask [B, *] (row stride mask_stride) is row b's own, not blended.
+ * loss_acc[0] += mean over all B*C elements of mask * BCE(z, y_mix); dlogits (optional) = mask * (sigmoid(z) - y_mix) / (B*C).
+ * y_stride, mask_stride >= C (y = batch[:, :C] and mask = batch[:, C:] of one [B, 2C] tensor: stride 2C). */
+int eat_bce_masked_loss(const float* logits, const float* y, int y_stride, const float* mask, int mask_stride,
+                        const int* perm, const float* lam, int B, int C, float* dlogits, double* loss_acc,
+                        cudaStream_t stream);
+/* Frequency-wise MixStyle, helpers/utils.py:101-121, on x [B, 1, F, T] fp32 (out of place, out [B, 1, F, T]):
+ * mu, sig = mean and sqrt(unbiased variance + eps) over T per (b, f) (two passes over each row, fp32);
+ * out = (x - mu_b) / sig_b * (lam_b sig_b + (1 - lam_b) sig_pb) + lam_b mu_b + (1 - lam_b) mu_pb with pb = perm[b].
+ * stats: workspace of 2*B*F floats (mu, sig per row).  Two launches: statistics, then apply.  T >= 2, else EAT_ERR_ARG. */
+int eat_mixstyle(const float* x, const int* perm, const float* lam, float eps, float* stats, float* out, int B, int F,
+                 int T, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
