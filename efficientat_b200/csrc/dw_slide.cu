@@ -14,6 +14,7 @@
 // No shared-memory staging of activations and no CTA barriers in the main loop; weights sit in shared memory.
 //
 // Algorithmic bytes: B*F*T*C + B*Fo*To*C elements (+ residual in the data-gradient mode), HBM bound.
+#include <cstdio>
 #include <cstdlib>
 #include <type_traits>
 
@@ -95,8 +96,12 @@ struct SlideArgs {
 // MODE 0: training forward (optional input BN+act XACT >= 0, raw output + batch statistics)
 // MODE 1: eval forward (folded BN + act epilogue, SE pooling, DyMN DyReLU-B / coordinate attention)
 // MODE 2: stride-1 data gradient (mirrored taps, optional residual-gradient add)
-template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, bool RING>
+// D = 2: dilation 2 at stride 1.  Such a layer is four independent undilated K x K convolutions, one on each (row parity,
+// column parity) sub-grid of the image, so a unit walks rows and columns of one parity: the same walk with row and column
+// steps of two pixels.  Each sample has D * D times the units of one sub-grid; D = 1 is the undilated kernel.
+template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, bool RING, int D = 1>
 __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) {
+  static_assert(D == 1 || (D == 2 && S == 1), "dilation 2 is stride 1 only");
   constexpr int V = Vec<T>::N;
   constexpr int NIN = (P - 1) * S + K, PAD = (K - 1) / 2, KK = K * K;
   constexpr int L = (K + S - 1) / S;           // output rows alive at once
@@ -162,15 +167,19 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
     const T* inb = nullptr;
     T* outb = nullptr;
     const T* resb = nullptr;
-    const int strips = ceil_div(To, P), segs = ceil_div(Fo, a.seg_rows), units = strips * segs;
-    const long long rowstride = (long long)Tn * C;
+    // D = 2: strips and segments of the largest sub-grid, ceil(Fo / 2) x ceil(To / 2)
+    const int strips = ceil_div(D == 1 ? To : (To + 1) / 2, P), segs = ceil_div(D == 1 ? Fo : (Fo + 1) / 2, a.seg_rows);
+    const int units = D * D * strips * segs;
+    const long long rowstride = (long long)Tn * C * D;
+    const int cstep = C * D;                     // elements between the columns a unit reads
+    int Fs = Fo, Ts = To;                        // rows / columns of the unit's sub-grid (D = 1: the image)
 
     // epilogue of one finished output row (P vectors), then the row is stored
     auto finish = [&](float (&o)[P][V], int fo, int to0) {
 #pragma unroll
       for (int p = 0; p < P; ++p) {
         const int to = to0 + p;
-        if (to < To) {
+        if (to < Ts) {
           if (kAff && a.scale != nullptr) {
 #pragma unroll
             for (int i = 0; i < V; ++i) { o[p][i] = act_fwd(fmaf(o[p][i], osc[i], osh[i]), a.act); lsum[i] += o[p][i]; }
@@ -192,7 +201,7 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
               o[p][4 * q + 2] *= f4.z * t4.z; o[p][4 * q + 3] *= f4.w * t4.w;
             }
           }
-          const size_t off = ((size_t)fo * To + to) * C;
+          const size_t off = D == 1 ? ((size_t)fo * To + to) * C : ((size_t)(D * fo) * To + D * to) * C;
           if (kRes && resb != nullptr) {
             float r[V];
             Vec<T>::load(resb + off, r);
@@ -210,20 +219,32 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
     const long long gstep = a.per_sample ? (long long)groups * ppb : (long long)gridDim.y * groups * ppb;
     for (; g < gend; g += gstep) {
       bb = (int)(g / units);
-      const int u = (int)(g - (long long)bb * units);
+      int u = (int)(g - (long long)bb * units);
       inb = reinterpret_cast<const T*>(a.in) + (size_t)bb * F * Tn * C + c0;
       outb = reinterpret_cast<T*>(a.out) + (size_t)bb * Fo * To * C + c0;
       if (kRes && a.res != nullptr) resb = reinterpret_cast<const T*>(a.res) + (size_t)bb * Fo * To * C + c0;
+      if constexpr (D == 2) {                               // sub-grid (pr, pc): image rows pr, pr+2, .. and columns pc, pc+2, ..
+        const int par = u / (strips * segs), pr = par >> 1, pc = par & 1;
+        u -= par * strips * segs;
+        Fs = (Fo - pr + 1) >> 1;
+        Ts = (To - pc + 1) >> 1;
+        const size_t poff = ((size_t)pr * To + pc) * C;    // stride 1: input and output share the pixel grid
+        inb += poff;
+        outb += poff;
+        if (kRes && a.res != nullptr) resb += poff;
+      }
       const int seg = u / strips, strip = u - seg * strips;
       const int fo_a = seg * a.seg_rows;
-      const int nrows = min(a.seg_rows, Fo - fo_a);
+      const int nrows = min(a.seg_rows, Fs - fo_a);
       const int to0 = strip * P;
+      if (D == 2 && (nrows <= 0 || to0 >= Ts)) continue;    // past the end of a smaller sub-grid
       const int t0 = to0 * S - PAD;
+      const int Fin = D == 1 ? F : Fs, Tin = D == 1 ? Tn : Ts;
       unsigned cmask = 0;
 #pragma unroll
-      for (int j = 0; j < NIN; ++j) cmask |= (t0 + j >= 0 && t0 + j < Tn) ? (1u << j) : 0u;
+      for (int j = 0; j < NIN; ++j) cmask |= (t0 + j >= 0 && t0 + j < Tin) ? (1u << j) : 0u;
       const int i0 = fo_a * S - PAD;                        // input row of step 0
-      const T* colp = inb + (long long)t0 * C;              // column j of input row i: colp + i*rowstride + j*C
+      const T* colp = inb + (long long)t0 * cstep;          // column j of input row i: colp + i*rowstride + j*cstep
       float acc[L][P][V];
 #pragma unroll
       for (int l = 0; l < L; ++l)
@@ -239,12 +260,12 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
       auto issue = [&](int q, int slot_) {
         if (RING) {
           const int irow = i0 + q;
-          if (q < nfeed && irow >= 0 && irow < F) {
+          if (q < nfeed && irow >= 0 && irow < Fin) {
             const T* rp = colp + (long long)irow * rowstride;
             const uint32_t dst = ring0 + (uint32_t)(slot_ * NIN) * (kST * 16u);
 #pragma unroll
             for (int j = 0; j < NIN; ++j)
-              if ((cmask >> j) & 1u) cp_async<16>(dst + (uint32_t)j * (kST * 16u), rp + (size_t)j * C);
+              if ((cmask >> j) & 1u) cp_async<16>(dst + (uint32_t)j * (kST * 16u), rp + (size_t)j * cstep);
           }
           cp_commit();
         }
@@ -256,14 +277,14 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
       // one input row: load, transform once, scatter into the live output rows.  PH = row parity for S = 2.
       auto feed_row = [&](int irow, auto ph_tag) {
         constexpr int PH = decltype(ph_tag)::value;
-        if (irow < 0 || irow >= F) return;
+        if (irow < 0 || irow >= Fin) return;
         const T* rp = colp + (long long)irow * rowstride;
         float v[NIN][V];
 #pragma unroll
         for (int j = 0; j < NIN; ++j) {
           if ((cmask >> j) & 1u) {
             if (RING) Vec<T>::load(reinterpret_cast<const T*>(ringp + (size_t)(rs * NIN + j) * (kST * 16)), v[j]);
-            else Vec<T>::load(rp + (size_t)j * C, v[j]);
+            else Vec<T>::load(rp + (size_t)j * cstep, v[j]);
           } else {
 #pragma unroll
             for (int i = 0; i < V; ++i) v[j][i] = 0.f;
@@ -365,8 +386,9 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
 // candidate length and the cheapest wins.
 struct SlidePlan { int chunks, cvc, seg_rows, groups, gy; };
 
+// grids: independent sub-grids of Fo x To per sample (4 for a dilation-2 layer, see dw_slide_kernel)
 inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, int K, int ctas_per_sm, bool per_sample,
-                            int cvc_cap = kST) {
+                            int cvc_cap = kST, int grids = 1) {
   SlidePlan pl;
   const int cvc_max = min(kChMax / V < kST ? kChMax / V : kST, cvc_cap);
   pl.chunks = ceil_div(cv, cvc_max);
@@ -376,7 +398,7 @@ inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, 
   const long long ctas = (long long)kNumSMs * ctas_per_sm;
   // CTAs available to one channel chunk (per sample when blockIdx.y must be the sample)
   const long long lanes = per_sample ? max(1LL, ctas / ((long long)B * pl.chunks)) : max(1LL, ctas / pl.chunks);
-  const long long work_items = per_sample ? 1 : B;
+  const long long work_items = (per_sample ? 1LL : (long long)B) * grids;
   // makespan model: rounds of units per thread slot x row steps per unit (segment rows + the L-1 halo steps)
   const int L = (K + S - 1) / S;
   const long long slots = lanes * ppb;
@@ -387,7 +409,7 @@ inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, 
     const long long cost = ((units + slots - 1) / slots) * (seg + L - 1);
     if (best < 0 || cost < best) { best = cost; pl.seg_rows = seg; }
   }
-  const long long units1 = (long long)strips * ceil_div(Fo, pl.seg_rows);     // units of one sample
+  const long long units1 = (long long)strips * ceil_div(Fo, pl.seg_rows) * grids;     // units of one sample
   if (per_sample) {
     pl.gy = B;
     pl.groups = (int)min(lanes, (long long)ceil_div((int)units1, ppb));
@@ -400,42 +422,42 @@ inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, 
   return pl;
 }
 
-template <typename T, int K, int S, int P, int MODE, int XACT, int MINB>
+template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, int D = 1>
 void launch_one(SlideArgs a, dim3 grid, size_t smem, cudaStream_t st) {
   constexpr int NIN = (P - 1) * S + K;
   const size_t slot = (size_t)NIN * kST * 16;
   a.depth = ring_depth((size_t)(227 * 1024) / MINB - 1024, smem, slot, a.cvc * Vec<T>::N <= 32 ? 3 : 2);
   static unsigned long long mask0 = 0, mask1 = 0;
   if (a.depth > 0) {
-    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, true>;
+    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, true, D>;
     if (eat_opt_in_smem(kern, 200 * 1024, mask1) != EAT_OK) return;
     kern<<<grid, kST, smem + a.depth * slot, st>>>(a);
   } else {
-    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, false>;
+    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, false, D>;
     if (eat_opt_in_smem(kern, 64 * 1024, mask0) != EAT_OK) return;
     kern<<<grid, kST, smem, st>>>(a);
   }
 }
 
-template <typename T, int K, int S, int P, int MINB>
+template <typename T, int K, int S, int P, int MINB, int D = 1>
 int launch_mode(const SlideArgs& a, int mode, int xact_code, dim3 grid, size_t smem, cudaStream_t st) {
-  if (mode == 1) launch_one<T, K, S, P, 1, -1, MINB>(a, grid, smem, st);
+  if (mode == 1) launch_one<T, K, S, P, 1, -1, MINB, D>(a, grid, smem, st);
   else if (mode == 2) {
     if (S != 1) { eat_set_error("dw slide: data-gradient mode is stride 1 only"); return EAT_ERR_UNSUPPORTED; }
-    launch_one<T, K, 1, P, 2, -1, MINB>(a, grid, smem, st);
+    launch_one<T, K, 1, P, 2, -1, MINB, D>(a, grid, smem, st);
   } else {
     switch (xact_code) {
-      case -1: launch_one<T, K, S, P, 0, -1, MINB>(a, grid, smem, st); break;
-      case EAT_ACT_NONE: launch_one<T, K, S, P, 0, EAT_ACT_NONE, MINB>(a, grid, smem, st); break;
-      case EAT_ACT_RELU: launch_one<T, K, S, P, 0, EAT_ACT_RELU, MINB>(a, grid, smem, st); break;
-      case EAT_ACT_HSWISH: launch_one<T, K, S, P, 0, EAT_ACT_HSWISH, MINB>(a, grid, smem, st); break;
+      case -1: launch_one<T, K, S, P, 0, -1, MINB, D>(a, grid, smem, st); break;
+      case EAT_ACT_NONE: launch_one<T, K, S, P, 0, EAT_ACT_NONE, MINB, D>(a, grid, smem, st); break;
+      case EAT_ACT_RELU: launch_one<T, K, S, P, 0, EAT_ACT_RELU, MINB, D>(a, grid, smem, st); break;
+      case EAT_ACT_HSWISH: launch_one<T, K, S, P, 0, EAT_ACT_HSWISH, MINB, D>(a, grid, smem, st); break;
       default: eat_set_error("dw slide: unsupported input activation"); return EAT_ERR_UNSUPPORTED;
     }
   }
   return EAT_OK;
 }
 
-template <typename T>
+template <typename T, int D = 1>
 int launch_slide(SlideArgs a, int B, int k, int stride, int mode, int xact_code, cudaStream_t st) {
   constexpr int V = Vec<T>::N;
   constexpr bool kF32 = V == 4;
@@ -446,12 +468,17 @@ int launch_slide(SlideArgs a, int B, int k, int stride, int mode, int xact_code,
   const int minb = k == 3 ? (stride == 1 ? 4 : 5) : 3;
   a.B = B;
   a.per_sample = (a.pool != nullptr || a.dy.theta != nullptr || a.dy.ca_f != nullptr || a.dy.wt_bstride != 0) ? 1 : 0;
-  const SlidePlan pl = plan_slide(B, a.Fo, a.To, cv, V, P, stride, k, minb, a.per_sample != 0);
+  const SlidePlan pl = plan_slide(B, ceil_div(a.Fo, D), ceil_div(a.To, D), cv, V, P, stride, k, minb, a.per_sample != 0, kST,
+                                  D * D);
   a.chunks = pl.chunks; a.cvc = pl.cvc; a.seg_rows = pl.seg_rows;
   dim3 grid(pl.chunks * pl.groups, pl.gy);
   const size_t smem = ((size_t)k * k + 2) * a.cvc * V * sizeof(float);
   int rc = EAT_OK;
-  if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4>(a, mode, xact_code, grid, smem, st);
+  if (D == 2) {
+    if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4, 2>(a, mode, xact_code, grid, smem, st);
+    else if (k == 5 && stride == 1) rc = launch_mode<T, 5, 1, kF32 ? 2 : 1, 3, 2>(a, mode, xact_code, grid, smem, st);
+    else { eat_set_error("dw slide: dilation 2 needs k in {3,5} and stride 1"); return EAT_ERR_UNSUPPORTED; }
+  } else if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4>(a, mode, xact_code, grid, smem, st);
   else if (k == 3 && stride == 2) rc = launch_mode<T, 3, 2, kF32 ? 2 : 1, 5>(a, mode, xact_code, grid, smem, st);
   else if (k == 5 && stride == 1) rc = launch_mode<T, 5, 1, kF32 ? 2 : 1, 3>(a, mode, xact_code, grid, smem, st);
   else if (k == 5 && stride == 2) rc = launch_mode<T, 5, 2, kF32 ? 2 : 1, 3>(a, mode, xact_code, grid, smem, st);
@@ -482,6 +509,14 @@ template <> struct VecW<float, 2> {
 template <> struct VecW<__nv_bfloat16, 8> {
   __device__ __forceinline__ static void load(const __nv_bfloat16* p, float (&v)[8]) { Vec<__nv_bfloat16>::load(p, v); }
 };
+template <> struct VecW<__nv_bfloat16, 4> {      // the dilated bf16 5x5 weight gradient: 25 x 4 tap accumulators
+  __device__ __forceinline__ static void load(const __nv_bfloat16* p, float (&v)[4]) {
+    const uint2 t = *reinterpret_cast<const uint2*>(p);
+    const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.x));
+    const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&t.y));
+    v[0] = lo.x; v[1] = lo.y; v[2] = hi.x; v[3] = hi.y;
+  }
+};
 
 struct WgArgs {
   const void* dz;
@@ -496,8 +531,10 @@ struct WgArgs {
   const float* xshift;
 };
 
-template <typename T, int K, int S, int P, int V, int XACT, int MINB, bool RING>
+// D = 2: dilation 2 at stride 1, walked sub-grid by sub-grid as in dw_slide_kernel
+template <typename T, int K, int S, int P, int V, int XACT, int MINB, bool RING, int D = 1>
 __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs a) {
+  static_assert(D == 1 || (D == 2 && S == 1), "dilation 2 is stride 1 only");
   constexpr int KK = K * K, PAD = (K - 1) / 2;
   constexpr int NIN = (P - 1) * S + K;
   constexpr int L = (K + S - 1) / S;
@@ -531,28 +568,42 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
     for (int q = 0; q < KK; ++q)
 #pragma unroll
       for (int i = 0; i < V; ++i) wacc[q][i] = 0.f;
-    const int strips = ceil_div(To, P), segs = ceil_div(Fo, a.seg_rows), units = strips * segs;
-    const long long rowstride = (long long)Tn * C;
+    const int strips = ceil_div(D == 1 ? To : (To + 1) / 2, P), segs = ceil_div(D == 1 ? Fo : (Fo + 1) / 2, a.seg_rows);
+    const int units = D * D * strips * segs;
+    const long long rowstride = (long long)Tn * C * D;
+    const int cstep = C * D;
     long long g = a.per_sample ? (long long)blockIdx.y * units + grp * ppb + slot : ((long long)blockIdx.y * groups + grp) * ppb + slot;
     const long long gend = a.per_sample ? (long long)(blockIdx.y + 1) * units : (long long)a.B * units;
     const long long gstep = a.per_sample ? (long long)groups * ppb : (long long)gridDim.y * groups * ppb;
     {
       for (; g < gend; g += gstep) {
         const int b = (int)(g / units);
-        const int u = (int)(g - (long long)b * units);
+        int u = (int)(g - (long long)b * units);
         const T* inb = reinterpret_cast<const T*>(a.in) + (size_t)b * F * Tn * C + c0;
         const T* dzb = reinterpret_cast<const T*>(a.dz) + (size_t)b * Fo * To * C + c0;
+        int Fs = Fo, Ts = To;                   // rows / columns of the unit's sub-grid (D = 1: the image)
+        if constexpr (D == 2) {
+          const int par = u / (strips * segs), pr = par >> 1, pc = par & 1;
+          u -= par * strips * segs;
+          Fs = (Fo - pr + 1) >> 1;
+          Ts = (To - pc + 1) >> 1;
+          const size_t poff = ((size_t)pr * To + pc) * C;
+          inb += poff;
+          dzb += poff;
+        }
         const int seg = u / strips, strip = u - seg * strips;
         const int fo_a = seg * a.seg_rows;
-        const int nrows = min(a.seg_rows, Fo - fo_a);
+        const int nrows = min(a.seg_rows, Fs - fo_a);
         const int to0 = strip * P;
+        if (D == 2 && (nrows <= 0 || to0 >= Ts)) continue;
         const int t0 = to0 * S - PAD;
+        const int Fin = D == 1 ? F : Fs, Tin = D == 1 ? Tn : Ts;
         unsigned cmask = 0;
 #pragma unroll
-        for (int j = 0; j < NIN; ++j) cmask |= (t0 + j >= 0 && t0 + j < Tn) ? (1u << j) : 0u;
+        for (int j = 0; j < NIN; ++j) cmask |= (t0 + j >= 0 && t0 + j < Tin) ? (1u << j) : 0u;
         const int i0 = fo_a * S - PAD;
-        const T* colp = inb + (long long)t0 * C;
-        const T* dzp = dzb + ((size_t)fo_a * To + to0) * C;
+        const T* colp = inb + (long long)t0 * cstep;
+        const T* dzp = dzb + (D == 1 ? ((size_t)fo_a * To + to0) * C : ((size_t)(D * fo_a) * To + D * to0) * C);
         float dzw[L][P][V];
 #pragma unroll
         for (int l = 0; l < L; ++l)
@@ -570,7 +621,7 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
           const T* rp = colp + (long long)irow * rowstride;
 #pragma unroll
           for (int j = 0; j < NIN; ++j) {
-            if ((cmask >> j) & 1u) VecW<T, V>::load(rp + (size_t)j * C, v[j]);
+            if ((cmask >> j) & 1u) VecW<T, V>::load(rp + (size_t)j * cstep, v[j]);
             else {
 #pragma unroll
               for (int i = 0; i < V; ++i) v[j][i] = 0.f;
@@ -617,10 +668,10 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
 #pragma unroll
               for (int i = 0; i < V; ++i) dzw[l][p][i] = dzw[l + 1][p][i];
           if (n < nrows) {
-            const T* gp = dzp + (size_t)n * To * C;
+            const T* gp = dzp + (size_t)n * To * C * D;
 #pragma unroll
             for (int p = 0; p < P; ++p) {
-              if (to0 + p < To) VecW<T, V>::load(gp + (size_t)p * C, dzw[L - 1][p]);
+              if (to0 + p < Ts) VecW<T, V>::load(gp + (size_t)p * cstep, dzw[L - 1][p]);
               else {
 #pragma unroll
                 for (int i = 0; i < V; ++i) dzw[L - 1][p][i] = 0.f;
@@ -638,17 +689,17 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
           // cp.async group into slot n % depth; the thread reads back only its own copies
           auto rows_of = [&](int n, int& ie, bool& ev, bool& od) {
             ie = i0 + n * S;
-            ev = ie >= 0 && ie < F;
-            od = S == 2 && (n < nrows + (K - 3) / 2) && ie + 1 >= 0 && ie + 1 < F;
+            ev = ie >= 0 && ie < Fin;
+            od = S == 2 && (n < nrows + (K - 3) / 2) && ie + 1 >= 0 && ie + 1 < Fin;
           };
           auto issue = [&](int n, int slot_) {
             if (n < steps) {
               const uint32_t dst = ring0 + (uint32_t)(slot_ * NV) * (kST * VB);
               if (n < nrows) {
-                const T* gp = dzp + (size_t)n * To * C;
+                const T* gp = dzp + (size_t)n * To * C * D;
 #pragma unroll
                 for (int p = 0; p < P; ++p)
-                  if (to0 + p < To) cp_async<VB>(dst + (uint32_t)p * (kST * VB), gp + (size_t)p * C);
+                  if (to0 + p < Ts) cp_async<VB>(dst + (uint32_t)p * (kST * VB), gp + (size_t)p * cstep);
               }
               int ie; bool ev, od;
               rows_of(n, ie, ev, od);
@@ -656,13 +707,13 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
                 const T* rp = colp + (long long)ie * rowstride;
 #pragma unroll
                 for (int j = 0; j < NIN; ++j)
-                  if ((cmask >> j) & 1u) cp_async<VB>(dst + (uint32_t)(P + j) * (kST * VB), rp + (size_t)j * C);
+                  if ((cmask >> j) & 1u) cp_async<VB>(dst + (uint32_t)(P + j) * (kST * VB), rp + (size_t)j * cstep);
               }
               if (od) {
                 const T* rp = colp + (long long)(ie + 1) * rowstride;
 #pragma unroll
                 for (int j = 0; j < NIN; ++j)
-                  if ((cmask >> j) & 1u) cp_async<VB>(dst + (uint32_t)(P + NIN + j) * (kST * VB), rp + (size_t)j * C);
+                  if ((cmask >> j) & 1u) cp_async<VB>(dst + (uint32_t)(P + NIN + j) * (kST * VB), rp + (size_t)j * cstep);
               }
             }
             cp_commit();
@@ -689,7 +740,7 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
                 for (int i = 0; i < V; ++i) dzw[l][p][i] = dzw[l + 1][p][i];
 #pragma unroll
             for (int p = 0; p < P; ++p) {
-              if (n < nrows && to0 + p < To) VecW<T, V>::load(reinterpret_cast<const T*>(ringp + (size_t)(rs * NV + p) * (kST * VB)), dzw[L - 1][p]);
+              if (n < nrows && to0 + p < Ts) VecW<T, V>::load(reinterpret_cast<const T*>(ringp + (size_t)(rs * NV + p) * (kST * VB)), dzw[L - 1][p]);
               else {
 #pragma unroll
                 for (int i = 0; i < V; ++i) dzw[L - 1][p][i] = 0.f;
@@ -718,10 +769,10 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
           auto step = [&](int n, auto cur, auto nxt) {
             slide_window(n);
             const int ie = i0 + n;
-            if (n + 1 < steps && ie + 1 >= 0 && ie + 1 < F) ld(ie + 1, nxt);
-            if (ie >= 0 && ie < F) mac(cur, Ph0{});
+            if (n + 1 < steps && ie + 1 >= 0 && ie + 1 < Fin) ld(ie + 1, nxt);
+            if (ie >= 0 && ie < Fin) mac(cur, Ph0{});
           };
-          if (i0 >= 0 && i0 < F) ld(i0, Ph0{});
+          if (i0 >= 0 && i0 < Fin) ld(i0, Ph0{});
           for (int n = 0; n < steps; n += 2) {
             step(n, Ph0{}, Ph1{});
             if (n + 1 < steps) step(n + 1, Ph1{}, Ph0{});
@@ -742,44 +793,48 @@ __global__ void __launch_bounds__(kST, MINB) dw_wgrad_slide_kernel(const WgArgs 
   }
 }
 
-template <typename T, int K, int S, int P, int V, int XACT, int MINB>
+template <typename T, int K, int S, int P, int V, int XACT, int MINB, int D>
 int launch_wg_one(WgArgs a, dim3 grid, size_t smem, cudaStream_t st) {
   constexpr int NIN = (P - 1) * S + K;
   const size_t slot = (size_t)(P + NIN * S) * kST * V * sizeof(T);
   a.depth = ring_depth((size_t)(227 * 1024) / MINB - 1024, smem, slot, S == 1 ? 2 : 0);   // stride 2: a slot holds two input rows, the ring costs a CTA
   static unsigned long long mask1 = 0;
   if (a.depth > 0) {
-    auto kern = dw_wgrad_slide_kernel<T, K, S, P, V, XACT, MINB, true>;
+    auto kern = dw_wgrad_slide_kernel<T, K, S, P, V, XACT, MINB, true, D>;
     if (int rc = eat_opt_in_smem(kern, 200 * 1024, mask1)) return rc;
     kern<<<grid, kST, smem + a.depth * slot, st>>>(a);
   } else {
-    dw_wgrad_slide_kernel<T, K, S, P, V, XACT, MINB, false><<<grid, kST, smem, st>>>(a);
+    dw_wgrad_slide_kernel<T, K, S, P, V, XACT, MINB, false, D><<<grid, kST, smem, st>>>(a);
   }
   return EAT_OK;
 }
 
-template <typename T, int K, int S, int P, int V, int MINB>
+template <typename T, int K, int S, int P, int V, int MINB, int D = 1>
 int launch_wg_act(const WgArgs& a, int xact_code, dim3 grid, size_t smem, cudaStream_t st) {
   switch (xact_code) {
-    case -1: return launch_wg_one<T, K, S, P, V, -1, MINB>(a, grid, smem, st);
-    case EAT_ACT_NONE: return launch_wg_one<T, K, S, P, V, EAT_ACT_NONE, MINB>(a, grid, smem, st);
-    case EAT_ACT_RELU: return launch_wg_one<T, K, S, P, V, EAT_ACT_RELU, MINB>(a, grid, smem, st);
-    case EAT_ACT_HSWISH: return launch_wg_one<T, K, S, P, V, EAT_ACT_HSWISH, MINB>(a, grid, smem, st);
+    case -1: return launch_wg_one<T, K, S, P, V, -1, MINB, D>(a, grid, smem, st);
+    case EAT_ACT_NONE: return launch_wg_one<T, K, S, P, V, EAT_ACT_NONE, MINB, D>(a, grid, smem, st);
+    case EAT_ACT_RELU: return launch_wg_one<T, K, S, P, V, EAT_ACT_RELU, MINB, D>(a, grid, smem, st);
+    case EAT_ACT_HSWISH: return launch_wg_one<T, K, S, P, V, EAT_ACT_HSWISH, MINB, D>(a, grid, smem, st);
     default: eat_set_error("dw wgrad slide: unsupported input activation"); return EAT_ERR_UNSUPPORTED;
   }
 }
 
 // K = 3: 4 fp32 (8 bf16) channels per thread; K = 5 (fp32 only): 2 channels per thread, 25 x 2 tap accumulators
-template <typename T, int K, int V, int P, int MINB>
+template <typename T, int K, int V, int P, int MINB, int D = 1>
 int launch_wg_slide(WgArgs a, int stride, int xact_code, cudaStream_t st) {
   const int cv = a.C / V;
   a.per_sample = a.dw_bstride != 0 ? 1 : 0;
-  const SlidePlan pl = plan_slide(a.B, a.Fo, a.To, cv, V, P, stride, K, stride == 2 ? 3 : MINB, a.per_sample != 0);
+  const SlidePlan pl = plan_slide(a.B, ceil_div(a.Fo, D), ceil_div(a.To, D), cv, V, P, stride, K, stride == 2 ? 3 : MINB,
+                                  a.per_sample != 0, kST, D * D);
   a.chunks = pl.chunks; a.cvc = pl.cvc; a.seg_rows = pl.seg_rows;
   dim3 grid(pl.chunks * pl.groups, pl.gy);
   const size_t smem = (size_t)K * K * a.cvc * V * sizeof(float);
   int rc;
-  if (stride == 1) rc = launch_wg_act<T, K, 1, P, V, MINB>(a, xact_code, grid, smem, st);
+  if (D == 2) {
+    if (stride != 1) { eat_set_error("dw wgrad slide: dilation 2 is stride 1 only"); return EAT_ERR_UNSUPPORTED; }
+    rc = launch_wg_act<T, K, 1, P, V, MINB, 2>(a, xact_code, grid, smem, st);
+  } else if (stride == 1) rc = launch_wg_act<T, K, 1, P, V, MINB>(a, xact_code, grid, smem, st);
   else rc = launch_wg_act<T, K, 2, P, V, 3>(a, xact_code, grid, smem, st);     // two row buffers: 168 registers
   if (rc != EAT_OK) return rc;
   EAT_CHECK_LAUNCH();
@@ -1507,46 +1562,130 @@ extern "C" int eat_dw_conv_bwd_fused(const float* dp, const float* gate, const f
   return stride == 1 ? launch_fb<5, 1>(a, act, xf, st) : launch_fb<5, 2>(a, act, xf, st);
 }
 
-int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
-                    InXform xf, const float* scale, const float* shift, int act, const void* res, int flip, float* pool,
-                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy) {
+namespace {
+// dil 2 (stride 1, padding 2 * (k-1)/2): the output has the input's size
+int slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
+                 int dil, InXform xf, const float* scale, const float* shift, int act, const void* res, int flip,
+                 float* pool, double* ssum, double* ssq, cudaStream_t st, DyEpi dy) {
   const int V = dtype == EAT_BF16 ? 8 : 4;
   if (C % V != 0) { eat_set_error("dw conv: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
-  const int pad = (k - 1) / 2;
+  const int pad = (k - 1) / 2 * dil;
   SlideArgs a;
   a.in = in; a.wt = wt; a.out = out;
   a.F = F; a.Tn = Tn; a.C = C;
-  a.Fo = (F + 2 * pad - k) / stride + 1;
-  a.To = (Tn + 2 * pad - k) / stride + 1;
+  a.Fo = (F + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  a.To = (Tn + 2 * pad - dil * (k - 1) - 1) / stride + 1;
   a.xscale = xf.scale; a.xshift = xf.shift;
   a.scale = scale; a.shift = shift; a.act = act;
   a.res = res; a.flip = flip; a.pool = pool; a.stat_sum = ssum; a.stat_sq = ssq; a.dy = dy;
   const int mode = (scale != nullptr || pool != nullptr || dy.theta != nullptr || dy.ca_f != nullptr) ? 1 : ((flip || res != nullptr) ? 2 : 0);
   const int xact_code = xf.scale != nullptr ? xf.act : -1;
   if (mode != 0 && xf.scale != nullptr) { eat_set_error("dw slide: input transform only in training-forward mode"); return EAT_ERR_UNSUPPORTED; }
+  if (dil == 2) {
+    if (dtype == EAT_BF16) return launch_slide<__nv_bfloat16, 2>(a, B, k, stride, mode, xact_code, st);
+    return launch_slide<float, 2>(a, B, k, stride, mode, xact_code, st);
+  }
   if (dtype == EAT_BF16) return launch_slide<__nv_bfloat16>(a, B, k, stride, mode, xact_code, st);
   return launch_slide<float>(a, B, k, stride, mode, xact_code, st);
 }
 
-int dw_wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
-                          int F, int Tn, int C, int k, int stride, cudaStream_t st) {
+int wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
+                       int F, int Tn, int C, int k, int stride, int dil, cudaStream_t st) {
   const int V = dtype == EAT_BF16 ? 8 : 4;
   if (C % V != 0) { eat_set_error("dw wgrad: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
-  if (!((k == 3 || (k == 5 && dtype != EAT_BF16)) && (stride == 1 || stride == 2))) {
+  if (dil == 1 && !((k == 3 || (k == 5 && dtype != EAT_BF16)) && (stride == 1 || stride == 2))) {
     eat_set_error("dw wgrad slide: 3x3 (fp32, bf16) or 5x5 (fp32), stride 1 or 2");
     return EAT_ERR_UNSUPPORTED;
   }
-  const int pad = (k - 1) / 2;
+  const int pad = (k - 1) / 2 * dil;
   WgArgs a;
   a.dz = dz; a.in = in; a.dw = dw; a.dw_bstride = dw_bstride;
   a.B = B; a.F = F; a.Tn = Tn; a.C = C;
-  a.Fo = (F + 2 * pad - k) / stride + 1;
-  a.To = (Tn + 2 * pad - k) / stride + 1;
+  a.Fo = (F + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  a.To = (Tn + 2 * pad - dil * (k - 1) - 1) / stride + 1;
   a.xscale = xf.scale; a.xshift = xf.shift;
   const int xact_code = xf.scale != nullptr ? xf.act : -1;
+  if (dil == 2) {          // the bf16 5x5 instance takes 4 channels per thread: 25 x 8 accumulators would spill
+    if (dtype == EAT_BF16) return k == 5 ? launch_wg_slide<__nv_bfloat16, 5, 4, 1, 3, 2>(a, stride, xact_code, st)
+                                         : launch_wg_slide<__nv_bfloat16, 3, 8, 1, 3, 2>(a, stride, xact_code, st);
+    if (k == 5) return launch_wg_slide<float, 5, 2, 4, 3, 2>(a, stride, xact_code, st);
+    return launch_wg_slide<float, 3, 4, 4, 3, 2>(a, stride, xact_code, st);
+  }
   if (dtype == EAT_BF16) return launch_wg_slide<__nv_bfloat16, 3, 8, 1, 3>(a, stride, xact_code, st);
   if (k == 5) return launch_wg_slide<float, 5, 2, 4, 3>(a, stride, xact_code, st);
   return launch_wg_slide<float, 3, 4, 4, 3>(a, stride, xact_code, st);
+}
+
+// argument checks of the dilated entry points, before any launch
+int dil_check(const char* who, int dtype, int B, int F, int T, int C, int k, int stride, int dilation) {
+  char msg[160];
+  int rc = EAT_OK;
+  if (dtype != EAT_F32 && dtype != EAT_BF16) { snprintf(msg, sizeof msg, "%s: dtype must be fp32 (0) or bf16 (1)", who); rc = EAT_ERR_ARG; }
+  else if (B < 0 || F < 1 || T < 1 || C < 1) { snprintf(msg, sizeof msg, "%s: B >= 0 and F, T, C >= 1 required", who); rc = EAT_ERR_ARG; }
+  else if (dilation != 2) { snprintf(msg, sizeof msg, "%s: dilation must be 2 (got %d)", who, dilation); rc = EAT_ERR_UNSUPPORTED; }
+  else if (stride != 1) { snprintf(msg, sizeof msg, "%s: a dilated layer runs at stride 1 (got %d)", who, stride); rc = EAT_ERR_UNSUPPORTED; }
+  else if (k != 3 && k != 5) { snprintf(msg, sizeof msg, "%s: k must be 3 or 5 (got %d)", who, k); rc = EAT_ERR_UNSUPPORTED; }
+  else if (C % (dtype == EAT_BF16 ? 8 : 4) != 0) {
+    snprintf(msg, sizeof msg, "%s: C must be a multiple of %d for %s storage (got %d)", who, dtype == EAT_BF16 ? 8 : 4,
+             dtype == EAT_BF16 ? "bf16" : "fp32", C);
+    rc = EAT_ERR_ARG;
+  }
+  if (rc != EAT_OK) eat_set_error(msg);
+  return rc;
+}
+}  // namespace
+
+int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
+                    InXform xf, const float* scale, const float* shift, int act, const void* res, int flip, float* pool,
+                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy) {
+  return slide_launch(in, wt, out, dtype, B, F, Tn, C, k, stride, 1, xf, scale, shift, act, res, flip, pool, ssum, ssq, st, dy);
+}
+
+int dw_wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
+                          int F, int Tn, int C, int k, int stride, cudaStream_t st) {
+  return wgrad_slide_launch(dz, in, xf, dw, dw_bstride, dtype, B, F, Tn, C, k, stride, 1, st);
+}
+
+extern "C" int eat_dw_conv_fwd_dil(const void* in, const float* wt, void* out, int dtype, int B, int F, int T, int C, int k,
+                                   int stride, int dilation, const float* in_scale, const float* in_shift, int in_act,
+                                   const float* scale, const float* shift, int act, float* pool, double* stat_sum,
+                                   double* stat_sq, cudaStream_t st) {
+  if (int rc = dil_check("dw_conv_fwd_dil", dtype, B, F, T, C, k, stride, dilation)) return rc;
+  if (in_scale != nullptr && (scale != nullptr || pool != nullptr)) {
+    eat_set_error("dw_conv_fwd_dil: the input transform is for the training forward (no scale, shift or pool)");
+    return EAT_ERR_ARG;
+  }
+  if ((scale == nullptr) != (shift == nullptr) || (in_scale == nullptr) != (in_shift == nullptr) ||
+      (stat_sum == nullptr) != (stat_sq == nullptr)) {
+    eat_set_error("dw_conv_fwd_dil: scale/shift, in_scale/in_shift and stat_sum/stat_sq come in pairs");
+    return EAT_ERR_ARG;
+  }
+  if (B == 0) return EAT_OK;
+  InXform xf{in_scale, in_shift, nullptr, in_act, 0};
+  return slide_launch(in, wt, out, dtype, B, F, T, C, k, stride, dilation, xf, scale, shift, act, nullptr, 0, pool,
+                      stat_sum, stat_sq, st, DyEpi{nullptr, nullptr, nullptr, nullptr, nullptr, 0});
+}
+
+extern "C" int eat_dw_conv_dgrad_dil(const void* dz, const float* wt, const void* res, void* din, int dtype, int B, int F,
+                                     int T, int C, int k, int stride, int dilation, cudaStream_t st) {
+  if (int rc = dil_check("dw_conv_dgrad_dil", dtype, B, F, T, C, k, stride, dilation)) return rc;
+  if (B == 0) return EAT_OK;
+  InXform xf{nullptr, nullptr, nullptr, 0, 0};
+  return slide_launch(dz, wt, din, dtype, B, F, T, C, k, stride, dilation, xf, nullptr, nullptr, 0, res, 1, nullptr,
+                      nullptr, nullptr, st, DyEpi{nullptr, nullptr, nullptr, nullptr, nullptr, 0});
+}
+
+extern "C" int eat_dw_conv_wgrad_dil(const void* dz, const void* in, const float* in_scale, const float* in_shift,
+                                     int in_act, float* dw, int dtype, int B, int F, int T, int C, int k, int stride,
+                                     int dilation, cudaStream_t st) {
+  if (int rc = dil_check("dw_conv_wgrad_dil", dtype, B, F, T, C, k, stride, dilation)) return rc;
+  if ((in_scale == nullptr) != (in_shift == nullptr)) {
+    eat_set_error("dw_conv_wgrad_dil: in_scale and in_shift come in pairs");
+    return EAT_ERR_ARG;
+  }
+  if (B == 0) return EAT_OK;
+  InXform xf{in_scale, in_shift, nullptr, in_act, 0};
+  return wgrad_slide_launch(dz, in, xf, dw, 0, dtype, B, F, T, C, k, stride, dilation, st);
 }
 
 int dw_dgrad2_slide_launch(const void* dz, const float* wt, long long wt_bstride, const void* res, void* din, int dtype,

@@ -34,13 +34,13 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _conv_out(n, k, s):
-    return (n + 2 * ((k - 1) // 2) - k) // s + 1
+def _conv_out(n, k, s, d=1):
+    return (n + 2 * ((k - 1) // 2) * d - d * (k - 1) - 1) // s + 1
 
 
 class _Layer:
     """Plain record describing one block of the network for the launcher loops."""
-    pass
+    dil = 1             # depthwise dilation (MN's dilated tail: 2)
 
 
 # one pass instead of two over the SE blocks' expanded tensors; EAT_SE_FUSED=0 restores the two-pass route
@@ -180,7 +180,10 @@ class MNEngine:
             L.res = m.use_res_connect
             L.act = ACT["hswish"] if m.cnf.use_hs else ACT["relu"]
             L.k = m.cnf.kernel
-            L.stride = m.cnf.stride
+            # a dilated depthwise conv runs at stride 1 (reference block_types.py:150); dilated layers go to the
+            # eat_dw_conv_*_dil entry points, never to the fused depthwise backward or the dgrad + reduce kernel
+            L.dil = m.cnf.dilation
+            L.stride = 1 if L.dil > 1 else m.cnf.stride
             L.cin, L.cexp, L.cout = m.cnf.input_channels, m.cnf.expanded_channels, m.cnf.out_channels
             self.blocks.append(L)
         self.mha = self.model.classifier if isinstance(self.model.classifier, MultiHeadAttentionPooling) else None
@@ -340,13 +343,17 @@ class MNEngine:
                        act=blk.act)
         else:
             e = inp
-        Fo, To = _conv_out(Fi, blk.k, blk.stride), _conv_out(Ti, blk.k, blk.stride)
+        Fo, To = _conv_out(Fi, blk.k, blk.stride, blk.dil), _conv_out(Ti, blk.k, blk.stride, blk.dil)
         d = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         sc = self._fold(blk.dw[1], dev)
         pool = torch.zeros(B, blk.cexp, device=dev, dtype=torch.float32) if blk.se is not None else None
-        L.dw_conv_fwd(e.data_ptr(), self._dw_weights(blk.dw[0], dev).data_ptr(), d.data_ptr(), dc, B, Fi, Ti,
-                      blk.cexp, blk.k, blk.stride, 0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), blk.act,
-                      _ptr(pool), 0, 0, st)
+        wt = self._dw_weights(blk.dw[0], dev)
+        if blk.dil > 1:
+            L.dw_conv_fwd_dil(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, blk.dil,
+                              0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), blk.act, _ptr(pool), 0, 0, st)
+        else:
+            L.dw_conv_fwd(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, 0, 0, 0,
+                          sc[0].data_ptr(), sc[1].data_ptr(), blk.act, _ptr(pool), 0, 0, st)
         gate = None
         if blk.se is not None:
             gate, _ = self._se_gate(blk.se, pool, 1.0 / (Fo * To), B, blk.cexp, dev)
@@ -433,14 +440,19 @@ class MNEngine:
             dw_in, dw_sc = z1, sc1
         else:
             dw_in, dw_sc = inp, None
-        Fo, To = _conv_out(Fi, blk.k, blk.stride), _conv_out(Ti, blk.k, blk.stride)
+        Fo, To = _conv_out(Fi, blk.k, blk.stride, blk.dil), _conv_out(Ti, blk.k, blk.stride, blk.dil)
         Mo = B * Fo * To
         z2 = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         stt = self._new_stats(blk.cexp, dev)
         wt = self._dw_weights(blk.dw[0], dev)
-        L.dw_conv_fwd(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
-                      _ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
-                      blk.act if dw_sc is not None else 0, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+        xf = (_ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
+              blk.act if dw_sc is not None else 0)
+        if blk.dil > 1:
+            L.dw_conv_fwd_dil(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
+                              blk.dil, *xf, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+        else:
+            L.dw_conv_fwd(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, *xf,
+                          0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
         sc2, sv2 = self._finalize(blk.dw[1], stt, Mo, dev)
         R.update(z2=z2, sc2=sc2, sv2=sv2, wt=wt, Fo=Fo, To=To)
         gate = None
@@ -661,7 +673,7 @@ class MNEngine:
         has_exp = blk.expand is not None
         dw_in = R["z1"] if has_exp else R["inp"]
         sc1 = R["sc1"] if has_exp else None
-        if (self.dw_bwd_fused and dc == 0 and (blk.k, blk.stride) in DW_BWD_FUSED_SHAPES
+        if (self.dw_bwd_fused and dc == 0 and blk.dil == 1 and (blk.k, blk.stride) in DW_BWD_FUSED_SHAPES
                 and blk.cexp % (4 if blk.k == 3 else 2) == 0):      # the kernel's channel vector: 4 (3x3) or 2 (5x5)
             # dz2 is computed on load and never stored; one walk yields the depthwise input gradient, the depthwise
             # weight gradient and the expand BatchNorm's backward sums
@@ -680,13 +692,20 @@ class MNEngine:
             return self._expand_bwd(blk, R, dy, G, B, da1, sums1)
         dz2 = self._bn_bwd(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
                            G[blk.dw[1].weight], G[blk.dw[1].bias], dev, sums=sums2)
-        fork.run(lambda: L.dw_conv_wgrad(dz2.data_ptr(), dw_in.data_ptr(), _ptr(sc1[0]) if has_exp else 0,
-                                         _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0,
-                                         G[blk.dw[0].weight].data_ptr(), 0, dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
-                                         _stream()), dz2)
+        xf = (_ptr(sc1[0]) if has_exp else 0, _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0)
+        if blk.dil > 1:
+            fork.run(lambda: L.dw_conv_wgrad_dil(dz2.data_ptr(), dw_in.data_ptr(), *xf, G[blk.dw[0].weight].data_ptr(), dc,
+                                                 B, Fi, Ti, blk.cexp, blk.k, blk.stride, blk.dil, _stream()), dz2)
+        else:
+            fork.run(lambda: L.dw_conv_wgrad(dz2.data_ptr(), dw_in.data_ptr(), *xf, G[blk.dw[0].weight].data_ptr(), 0, dc,
+                                             B, Fi, Ti, blk.cexp, blk.k, blk.stride, _stream()), dz2)
         da1 = torch.empty_like(dw_in)
         sums1 = None
-        if has_exp and self.dgrad_bnred and blk.stride == 2 and dc == 0 and blk.k in (3, 5):
+        res = _ptr(dy) if (blk.res and not has_exp) else 0
+        if blk.dil > 1:
+            L.dw_conv_dgrad_dil(dz2.data_ptr(), R["wt"].data_ptr(), res, da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
+                                blk.stride, blk.dil, st)
+        elif has_exp and self.dgrad_bnred and blk.stride == 2 and dc == 0 and blk.k in (3, 5):
             # the expand BatchNorm's reduce pass rides in the epilogue of the kernel that produces its upstream gradient
             sums1 = self._zero_pool.take(2, blk.cexp, dev)
             L.dw_conv_dgrad_bnred(dz2.data_ptr(), R["wt"].data_ptr(), 0, da1.data_ptr(), R["z1"].data_ptr(),
@@ -695,8 +714,8 @@ class MNEngine:
                                   blk.cexp, blk.k, blk.stride, st)
         else:
             # without an expand stage the depthwise input IS the block input: fold the residual gradient in
-            L.dw_conv_dgrad(dz2.data_ptr(), R["wt"].data_ptr(), 0, _ptr(dy) if (blk.res and not has_exp) else 0,
-                            da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, st)
+            L.dw_conv_dgrad(dz2.data_ptr(), R["wt"].data_ptr(), 0, res, da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
+                            blk.stride, st)
         return self._expand_bwd(blk, R, dy, G, B, da1, sums1)
 
     def _expand_bwd(self, blk, R, dy, G, B, da1, sums1):

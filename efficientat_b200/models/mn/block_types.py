@@ -100,8 +100,8 @@ class InvertedResidual(FusedOnly):
         super().__init__()
         if not (1 <= cnf.stride <= 2):
             raise ValueError("illegal stride value")
-        if cnf.dilation != 1:
-            raise NotImplementedError("dilated depthwise convolutions are not implemented by the fused engine")
+        if cnf.dilation not in (1, 2):
+            raise NotImplementedError("the fused engine implements depthwise dilation 1 and 2 only")
         self.use_res_connect = cnf.stride == 1 and cnf.input_channels == cnf.out_channels
         layers: List[nn.Module] = []
         activation_layer = nn.Hardswish if cnf.use_hs else nn.ReLU
@@ -109,7 +109,8 @@ class InvertedResidual(FusedOnly):
             layers.append(ConvNormActivation(cnf.input_channels, cnf.expanded_channels, kernel_size=1,
                                              norm_layer=norm_layer, activation_layer=activation_layer))
         layers.append(ConvNormActivation(cnf.expanded_channels, cnf.expanded_channels, kernel_size=cnf.kernel,
-                                         stride=cnf.stride, dilation=cnf.dilation, groups=cnf.expanded_channels,
+                                         stride=1 if cnf.dilation > 1 else cnf.stride, dilation=cnf.dilation,
+                                         groups=cnf.expanded_channels,
                                          norm_layer=depthwise_norm_layer, activation_layer=activation_layer))
         if cnf.use_se and se_cnf is not None and se_cnf["se_dims"] is not None:
             layers.append(ConcurrentSEBlock(cnf.expanded_channels, cnf.f_dim, cnf.t_dim, se_cnf))

@@ -281,6 +281,22 @@ int eat_dw_conv_dgrad_bnred(const void* dz, const float* wt, const void* res, vo
 int eat_dw_conv_wgrad(const void* dz, const void* in, const float* in_scale, const float* in_shift, int in_act,
                       float* dw, long long dw_bstride, int dtype, int B, int F, int T, int C, int k, int stride,
                       cudaStream_t stream);   /* wt_bstride / dw_bstride: floats between per-sample tables (0: shared) */
+/* Dilated depthwise k x k conv, the tail of get_model(dilated=True) (models/mn/block_types.py:150-162 with
+ * cnf.dilation = 2): dilation 2, stride 1, padding (k-1)/2 * 2, so the output has the input's size [B,F,T,C].  The three
+ * entry points mirror eat_dw_conv_fwd (training forward with in_* applied on load and fp64 batch statistics, or the eval
+ * epilogue with folded BatchNorm + act and the SE squeeze sums into pool), the stride-1 data gradient of eat_dw_conv_dgrad
+ * (mirrored taps, din = data gradient of dz (+ res)) and eat_dw_conv_wgrad (dw [C,1,k,k] += weight gradient of dz against
+ * xf(in)).  wt is the tap-major table of eat_dw_repack.  dilation must be 2, stride 1, k 3 or 5, dtype fp32 or bf16, and
+ * C a multiple of 4 (fp32) or 8 (bf16); anything else returns EAT_ERR_ARG or EAT_ERR_UNSUPPORTED before any launch.
+ * B = 0 is a no-op. */
+int eat_dw_conv_fwd_dil(const void* in, const float* wt, void* out, int dtype, int B, int F, int T, int C, int k, int stride,
+                        int dilation, const float* in_scale, const float* in_shift, int in_act, const float* scale,
+                        const float* shift, int act, float* pool, double* stat_sum, double* stat_sq, cudaStream_t stream);
+int eat_dw_conv_dgrad_dil(const void* dz, const float* wt, const void* res, void* din, int dtype, int B, int F, int T,
+                          int C, int k, int stride, int dilation, cudaStream_t stream);
+int eat_dw_conv_wgrad_dil(const void* dz, const void* in, const float* in_scale, const float* in_shift, int in_act,
+                          float* dw, int dtype, int B, int F, int T, int C, int k, int stride, int dilation,
+                          cudaStream_t stream);
 /* The depthwise stage's backward in one pass, from the upstream gradient dp [B,Fo,To,C] of its BatchNorm + activation
  * (BN2, raw output z2 [B,Fo,To,C]) down to the input: dz = eat_bn_bwd_apply(dp, gate, dpool, z2, scale ... c2) is
  * computed on load and never stored; din [B,F,T,C] = data gradient of dz (+ res); dw [C,1,k,k] += weight gradient of
