@@ -99,18 +99,45 @@ struct InXform {
 };
 
 struct DyEpi {
-  const float* theta;    // [B, C, 4] sigmoid(coef_net(h_c)) or nullptr
-  const float* lam;      // [4] lambdas
-  const float* init;     // [4] init_v
+  const float* theta;    // [B, C, 2M] sigmoid(coef_net(h_c)) or nullptr (M = DyReLU-B pieces, 2 unless stated)
+  const float* lam;      // [2M] lambdas
+  const float* init;     // [2M] init_v
   const float* ca_f;     // [B, Fo, C] sigmoid(g_cf) or nullptr
   const float* ca_t;     // [B, To, C] sigmoid(g_ct)
   long long wt_bstride;  // floats between the weight tables of consecutive samples (0: shared weights)
 };
 
-// sliding-window depthwise convolution (dw_slide.cu); same contract as launch_dw in conv_kernels.cu
+// DyReLU-B with M linear pieces (dy_block.py:172-188) for one channel.  theta points at the channel's 2M values of
+// sigmoid(coef_net(h_c)), channel-major ([B, C, 2M]); a_m = (2 theta_m - 1) lam_m + init_m is the slope of piece m and
+// b_m = (2 theta_{M+m} - 1) lam_{M+m} + init_{M+m} its offset; out = max_m (a_m x + b_m).  The M = 2 kernels keep their
+// own four-register form; this one serves M = 1, 3, 4 (2M coefficients per channel in registers).
+template <int M>
+struct DyCoef {
+  float a[M], b[M];
+  __device__ __forceinline__ void load(const float* theta, const float* lam, const float* init) {
+#pragma unroll
+    for (int m = 0; m < M; ++m) {
+      a[m] = (2.f * __ldg(theta + m) - 1.f) * __ldg(lam + m) + __ldg(init + m);
+      b[m] = (2.f * __ldg(theta + M + m) - 1.f) * __ldg(lam + M + m) + __ldg(init + M + m);
+    }
+  }
+  __device__ __forceinline__ void zero() {
+#pragma unroll
+    for (int m = 0; m < M; ++m) a[m] = b[m] = 0.f;
+  }
+  __device__ __forceinline__ float apply(float x) const {
+    float o = fmaf(x, a[0], b[0]);
+#pragma unroll
+    for (int m = 1; m < M; ++m) o = fmaxf(o, fmaf(x, a[m], b[m]));
+    return o;
+  }
+};
+
+// sliding-window depthwise convolution (dw_slide.cu); same contract as launch_dw in conv_kernels.cu.  dyk: DyReLU-B
+// pieces of the eval epilogue (1..4; only read when dy.theta is set)
 int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
                     InXform xf, const float* scale, const float* shift, int act, const void* res, int flip, float* pool,
-                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy);
+                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy, int dyk = 2);
 
 int dw_wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
                           int F, int Tn, int C, int k, int stride, cudaStream_t st);

@@ -6,6 +6,7 @@
 // statistics (training).  Reference semantics: torchvision ConvNormActivation as used at
 // models/mn/model.py:125-133 and models/mn/block_types.py:140-170; SqueezeExcitation
 // models/mn/block_types.py:72-83.
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 
@@ -208,13 +209,17 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
 // ((FR-1)*S+K rows x (TT-1)*S+K columns x 32 channels) in shared memory as fp32, applying the producing layer's
 // BatchNorm + activation ONCE per element, then
 // every thread computes a strip of P outputs for one 4-channel vector from shared memory (LDS.128).
-template <typename T, int K, int S, int MODE>
-__global__ void __launch_bounds__(kThreads, 3) dw_tile_kernel(
+// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue (2: four registers; 1, 3, 4: DyCoef, common.cuh).  The 2 DM
+// coefficients per channel vector stay in registers: DM = 1 at 2 CTAs per SM, DM = 3, 4 at one (no spills; DESIGN.md
+// section 4)
+template <typename T, int K, int S, int MODE, int DM = 2>
+__global__ void __launch_bounds__(kThreads, DM == 2 ? 3 : (DM == 1 ? 2 : 1)) dw_tile_kernel(
     const T* __restrict__ in, const float* __restrict__ wt, T* __restrict__ out,
     int F, int Tn, int Fo, int To, int C, InXform xf,
     const float* __restrict__ scale, const float* __restrict__ shift, int act, const T* __restrict__ res, int flip,
     float* __restrict__ pool, double* __restrict__ stat_sum, double* __restrict__ stat_sq, DyEpi dy) {
   constexpr bool kAff = MODE == 1, kStats = MODE == 0, kXf = MODE == 0, kRes = MODE == 2, kDy = MODE == 1, kPool = MODE == 1;
+  static_assert(DM >= 1 && DM <= 4 && (DM == 2 || MODE == 1), "DyReLU-B pieces: 1..4, eval epilogue only");
   constexpr int VG = Vec<T>::N;                 // channels per 16-byte global vector
   constexpr int CC = 32;                        // channels per tile
   constexpr int CCV = CC / 4;
@@ -270,20 +275,26 @@ __global__ void __launch_bounds__(kThreads, 3) dw_tile_kernel(
   const bool cvalid = cvec < ccv_valid;
   float osc[4], osh[4], lsum[4] = {0.f, 0.f, 0.f, 0.f}, lsq[4] = {0.f, 0.f, 0.f, 0.f};
   float da1[4], da2[4], db1[4], db2[4];
+  DyCoef<DM> dyc[4];
   if (cvalid) {
     if (kAff && scale != nullptr) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) { osc[i] = scale[c0 + i]; osh[i] = shift[c0 + i]; }
     }
     if (kDy && dy.theta != nullptr) {
-      const float* th = dy.theta + ((size_t)b * C + c0) * 4;
+      if constexpr (DM == 2) {
+        const float* th = dy.theta + ((size_t)b * C + c0) * 4;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
-        da1[i] = (2.f * t4.x - 1.f) * dy.lam[0] + dy.init[0];
-        da2[i] = (2.f * t4.y - 1.f) * dy.lam[1] + dy.init[1];
-        db1[i] = (2.f * t4.z - 1.f) * dy.lam[2] + dy.init[2];
-        db2[i] = (2.f * t4.w - 1.f) * dy.lam[3] + dy.init[3];
+        for (int i = 0; i < 4; ++i) {
+          const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
+          da1[i] = (2.f * t4.x - 1.f) * dy.lam[0] + dy.init[0];
+          da2[i] = (2.f * t4.y - 1.f) * dy.lam[1] + dy.init[1];
+          db1[i] = (2.f * t4.z - 1.f) * dy.lam[2] + dy.init[2];
+          db2[i] = (2.f * t4.w - 1.f) * dy.lam[3] + dy.init[3];
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) dyc[i].load(dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), dy.lam, dy.init);
       }
     }
   }
@@ -360,8 +371,13 @@ __global__ void __launch_bounds__(kThreads, 3) dw_tile_kernel(
             }
           }
           if (kDy && dy.theta != nullptr) {
+            if constexpr (DM == 2) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) o[i] = fmaxf(fmaf(o[i], da1[i], db1[i]), fmaf(o[i], da2[i], db2[i]));
+              for (int i = 0; i < 4; ++i) o[i] = fmaxf(fmaf(o[i], da1[i], db1[i]), fmaf(o[i], da2[i], db2[i]));
+            } else {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) o[i] = dyc[i].apply(o[i]);
+            }
           }
           if (kDy && dy.ca_f != nullptr) {
             const float4 f4 = __ldg(reinterpret_cast<const float4*>(dy.ca_f + ((size_t)b * Fo + fo) * C + c0));
@@ -603,7 +619,7 @@ inline int grid_for(long long items, int per_block, int max_blocks = kNumSMs * 1
 template <typename T>
 int launch_dw(const T* in, const float* wt, T* out, int B, int F, int Tn, int C, int k, int stride, InXform xf,
               const float* scale, const float* shift, int act, const T* res, int flip, float* pool, double* ssum,
-              double* ssq, cudaStream_t st, DyEpi dy = DyEpi{nullptr, nullptr, nullptr, nullptr, nullptr, 0}) {
+              double* ssq, cudaStream_t st, DyEpi dy = DyEpi{nullptr, nullptr, nullptr, nullptr, nullptr, 0}, int dyk = 2) {
   constexpr int V = Vec<T>::N;
   if (C % V != 0) { eat_set_error("dw conv: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
   const int pad = (k - 1) / 2;
@@ -617,7 +633,7 @@ int launch_dw(const T* in, const float* wt, T* out, int B, int F, int Tn, int C,
   const bool slide5 = e5 != nullptr ? e5[0] == 's' : C <= 256;
   if ((stride == 1 || stride == 2) && (k == 3 || (k == 5 && (mode_ == 0 || (mode_ == 2 && slide5)))) && !(mode_ == 2 && stride != 1))
     return dw_slide_launch(in, wt, out, V == 8 ? EAT_BF16 : EAT_F32, B, F, Tn, C, k, stride, xf, scale, shift, act, res, flip,
-                           pool, ssum, ssq, st, dy);
+                           pool, ssum, ssq, st, dy, dyk);
   if (k != 5) { eat_set_error("dw conv: only k in {3,5}, stride in {1,2}"); return EAT_ERR_UNSUPPORTED; }
   // shared-memory tiled kernel: grid.x = channel chunks x tile groups (each CTA strides over its group's tiles)
   const int FR = stride == 1 ? 8 : 4, TT = stride == 1 ? 32 : 16;
@@ -629,17 +645,28 @@ int launch_dw(const T* in, const float* wt, T* out, int B, int F, int Tn, int C,
   dim3 grid(chunks * groups, B);
   size_t smem = ((size_t)IR * IT * 32 + (size_t)k * k * 32 + 64) * sizeof(float);
   const int tmode = (scale != nullptr || pool != nullptr || dy.theta != nullptr || dy.ca_f != nullptr) ? 1 : ((flip || res != nullptr) ? 2 : 0);
-#define EAT_DWM(KK, SS, MM)                                                                                     \
+#define EAT_DWM(KK, SS, MM, DK)                                                                                 \
   do {                                                                                                          \
     static unsigned long long attr = 0;                                                                         \
-    if (int rc = eat_opt_in_smem(dw_tile_kernel<T, KK, SS, MM>, 100 * 1024, attr)) return rc;                   \
-    dw_tile_kernel<T, KK, SS, MM><<<grid, kThreads, smem, st>>>(in, wt, out, F, Tn, Fo, To, C, xf, scale, shift, act, res, flip, pool, ssum, ssq, dy); \
+    if (int rc = eat_opt_in_smem(dw_tile_kernel<T, KK, SS, MM, DK>, 100 * 1024, attr)) return rc;               \
+    dw_tile_kernel<T, KK, SS, MM, DK><<<grid, kThreads, smem, st>>>(in, wt, out, F, Tn, Fo, To, C, xf, scale, shift, act, res, flip, pool, ssum, ssq, dy); \
   } while (0)
-#define EAT_DW(KK, SS) do { if (tmode == 0) EAT_DWM(KK, SS, 0); else if (tmode == 1) EAT_DWM(KK, SS, 1); else EAT_DWM(KK, SS, 2); } while (0)
+  // the eval epilogue's DyReLU-B pieces (dyk, only read when dy.theta is set)
+  const int tdk = (tmode == 1 && dy.theta != nullptr) ? dyk : 2;
+  if (tdk < 1 || tdk > 4) { eat_set_error("dw conv: DyReLU-B takes 1..4 linear pieces"); return EAT_ERR_UNSUPPORTED; }
+#define EAT_DW1(KK, SS)                                                                                         \
+  do {                                                                                                          \
+    if (tdk == 1) EAT_DWM(KK, SS, 1, 1);                                                                        \
+    else if (tdk == 3) EAT_DWM(KK, SS, 1, 3);                                                                   \
+    else if (tdk == 4) EAT_DWM(KK, SS, 1, 4);                                                                   \
+    else EAT_DWM(KK, SS, 1, 2);                                                                                 \
+  } while (0)
+#define EAT_DW(KK, SS) do { if (tmode == 0) EAT_DWM(KK, SS, 0, 2); else if (tmode == 1) EAT_DW1(KK, SS); else EAT_DWM(KK, SS, 2, 2); } while (0)
   if (k == 5 && stride == 1) EAT_DW(5, 1);
   else if (k == 5 && stride == 2) EAT_DW(5, 2);
   else { eat_set_error("dw conv: only k in {3,5}, stride in {1,2}"); return EAT_ERR_UNSUPPORTED; }
 #undef EAT_DWM
+#undef EAT_DW1
 #undef EAT_DW
   EAT_CHECK_LAUNCH();
   return EAT_OK;
@@ -707,6 +734,46 @@ int eat_dw_conv_fwd_dy(const void* in, const float* wt, long long wt_bstride, vo
   if (dtype == EAT_BF16)
     return launch_dw<__nv_bfloat16>((const __nv_bfloat16*)in, wt, (__nv_bfloat16*)out, B, F, T, C, k, stride, xf, scale, shift, 0, nullptr, 0, nullptr, stat_sum, stat_sq, st, dy);
   return launch_dw<float>((const float*)in, wt, (float*)out, B, F, T, C, k, stride, xf, scale, shift, 0, nullptr, 0, nullptr, stat_sum, stat_sq, st, dy);
+}
+
+// eat_dw_conv_fwd_dy with M DyReLU-B pieces: theta [B, C, 2M], lam / init [2M].  Every check comes before any launch.
+int eat_dw_conv_fwd_dy_m(const void* in, const float* wt, long long wt_bstride, void* out, int dtype, int B, int F, int T,
+                         int C, int k, int stride, const float* in_scale, const float* in_shift, int in_act,
+                         const float* scale, const float* shift, const float* theta, const float* lam,
+                         const float* init, const float* ca_f, const float* ca_t, int pieces, double* stat_sum,
+                         double* stat_sq, cudaStream_t st) {
+  char msg[192];
+  int rc = EAT_OK;
+  const bool eval = scale != nullptr || theta != nullptr || ca_f != nullptr;
+  if (dtype != EAT_F32 && dtype != EAT_BF16) { snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: dtype must be fp32 (0) or bf16 (1)"); rc = EAT_ERR_ARG; }
+  else if (B < 0 || F < 1 || T < 1 || C < 1) { snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: B >= 0 and F, T, C >= 1 required"); rc = EAT_ERR_ARG; }
+  else if (pieces < 1 || pieces > 4) {
+    snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: DyReLU-B takes 1..4 linear pieces (got %d)", pieces);
+    rc = EAT_ERR_UNSUPPORTED;
+  } else if (k != 3 && k != 5) { snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: k must be 3 or 5 (got %d)", k); rc = EAT_ERR_UNSUPPORTED; }
+  else if (stride != 1 && stride != 2) { snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: stride must be 1 or 2 (got %d)", stride); rc = EAT_ERR_UNSUPPORTED; }
+  else if (C % (dtype == EAT_BF16 ? 8 : 4) != 0) {
+    snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: C must be a multiple of %d for %s storage (got %d)", dtype == EAT_BF16 ? 8 : 4,
+             dtype == EAT_BF16 ? "bf16" : "fp32", C);
+    rc = EAT_ERR_ARG;
+  } else if ((scale == nullptr) != (shift == nullptr) || (in_scale == nullptr) != (in_shift == nullptr) ||
+             (stat_sum == nullptr) != (stat_sq == nullptr) || (ca_f == nullptr) != (ca_t == nullptr) ||
+             (theta == nullptr) != (lam == nullptr) || (theta == nullptr) != (init == nullptr)) {
+    snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: scale/shift, in_scale/in_shift, stat_sum/stat_sq, ca_f/ca_t and "
+             "theta/lam/init come in sets");
+    rc = EAT_ERR_ARG;
+  } else if (eval && (in_scale != nullptr || stat_sum != nullptr)) {
+    snprintf(msg, sizeof msg, "dw_conv_fwd_dy_m: the input transform and the statistics are for the training forward "
+             "(no scale, theta or ca_f)");
+    rc = EAT_ERR_ARG;
+  }
+  if (rc != EAT_OK) { eat_set_error(msg); return rc; }
+  if (B == 0) return EAT_OK;
+  InXform xf{in_scale, in_shift, nullptr, in_act, 0};
+  DyEpi dy{theta, lam, init, ca_f, ca_t, wt_bstride};
+  if (dtype == EAT_BF16)
+    return launch_dw<__nv_bfloat16>((const __nv_bfloat16*)in, wt, (__nv_bfloat16*)out, B, F, T, C, k, stride, xf, scale, shift, 0, nullptr, 0, nullptr, stat_sum, stat_sq, st, dy, pieces);
+  return launch_dw<float>((const float*)in, wt, (float*)out, B, F, T, C, k, stride, xf, scale, shift, 0, nullptr, 0, nullptr, stat_sum, stat_sq, st, dy, pieces);
 }
 
 // stride-1 depthwise data gradient = the forward kernel with mirrored taps (+ residual-gradient add)

@@ -99,9 +99,12 @@ struct SlideArgs {
 // D = 2: dilation 2 at stride 1.  Such a layer is four independent undilated K x K convolutions, one on each (row parity,
 // column parity) sub-grid of the image, so a unit walks rows and columns of one parity: the same walk with row and column
 // steps of two pixels.  Each sample has D * D times the units of one sub-grid; D = 1 is the undilated kernel.
-template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, bool RING, int D = 1>
+// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue.  DM = 2 is the four-register form; 1, 3 and 4 hold 2 DM coefficients
+// per channel in registers (DyCoef, common.cuh).
+template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, bool RING, int D = 1, int DM = 2>
 __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) {
   static_assert(D == 1 || (D == 2 && S == 1), "dilation 2 is stride 1 only");
+  static_assert(DM >= 1 && DM <= 4 && (DM == 2 || (MODE == 1 && D == 1)), "DyReLU-B pieces: 1..4, eval epilogue only");
   constexpr int V = Vec<T>::N;
   constexpr int NIN = (P - 1) * S + K, PAD = (K - 1) / 2, KK = K * K;
   constexpr int L = (K + S - 1) / S;           // output rows alive at once
@@ -149,15 +152,21 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
       for (int i = 0; i < V; ++i) { osc[i] = __ldg(a.scale + c0 + i); osh[i] = __ldg(a.shift + c0 + i); }
     }
     float da1[V], da2[V], db1[V], db2[V];
+    DyCoef<DM> dyc[V];
     if (kDy && a.dy.theta != nullptr) {
-      const float* th = a.dy.theta + ((size_t)b * C + c0) * 4;
+      if constexpr (DM == 2) {
+        const float* th = a.dy.theta + ((size_t)b * C + c0) * 4;
 #pragma unroll
-      for (int i = 0; i < V; ++i) {
-        const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
-        da1[i] = (2.f * t4.x - 1.f) * a.dy.lam[0] + a.dy.init[0];
-        da2[i] = (2.f * t4.y - 1.f) * a.dy.lam[1] + a.dy.init[1];
-        db1[i] = (2.f * t4.z - 1.f) * a.dy.lam[2] + a.dy.init[2];
-        db2[i] = (2.f * t4.w - 1.f) * a.dy.lam[3] + a.dy.init[3];
+        for (int i = 0; i < V; ++i) {
+          const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
+          da1[i] = (2.f * t4.x - 1.f) * a.dy.lam[0] + a.dy.init[0];
+          da2[i] = (2.f * t4.y - 1.f) * a.dy.lam[1] + a.dy.init[1];
+          db1[i] = (2.f * t4.z - 1.f) * a.dy.lam[2] + a.dy.init[2];
+          db2[i] = (2.f * t4.w - 1.f) * a.dy.lam[3] + a.dy.init[3];
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < V; ++i) dyc[i].load(a.dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), a.dy.lam, a.dy.init);
       }
     }
     float lsum[V], lsq[V];
@@ -188,8 +197,13 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
             for (int i = 0; i < V; ++i) { lsum[i] += o[p][i]; lsq[i] = fmaf(o[p][i], o[p][i], lsq[i]); }
           }
           if (kDy && a.dy.theta != nullptr) {
+            if constexpr (DM == 2) {
 #pragma unroll
-            for (int i = 0; i < V; ++i) o[p][i] = fmaxf(fmaf(o[p][i], da1[i], db1[i]), fmaf(o[p][i], da2[i], db2[i]));
+              for (int i = 0; i < V; ++i) o[p][i] = fmaxf(fmaf(o[p][i], da1[i], db1[i]), fmaf(o[p][i], da2[i], db2[i]));
+            } else {
+#pragma unroll
+              for (int i = 0; i < V; ++i) o[p][i] = dyc[i].apply(o[p][i]);
+            }
           }
           if (kDy && a.dy.ca_f != nullptr) {
             const float* cf = a.dy.ca_f + ((size_t)bb * Fo + fo) * C + c0;
@@ -422,25 +436,43 @@ inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, 
   return pl;
 }
 
-template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, int D = 1>
+template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, int D = 1, int DM = 2>
 void launch_one(SlideArgs a, dim3 grid, size_t smem, cudaStream_t st) {
   constexpr int NIN = (P - 1) * S + K;
   const size_t slot = (size_t)NIN * kST * 16;
   a.depth = ring_depth((size_t)(227 * 1024) / MINB - 1024, smem, slot, a.cvc * Vec<T>::N <= 32 ? 3 : 2);
   static unsigned long long mask0 = 0, mask1 = 0;
   if (a.depth > 0) {
-    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, true, D>;
+    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, true, D, DM>;
     if (eat_opt_in_smem(kern, 200 * 1024, mask1) != EAT_OK) return;
     kern<<<grid, kST, smem + a.depth * slot, st>>>(a);
   } else {
-    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, false, D>;
+    auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, false, D, DM>;
     if (eat_opt_in_smem(kern, 64 * 1024, mask0) != EAT_OK) return;
     kern<<<grid, kST, smem, st>>>(a);
   }
 }
 
+// the eval epilogue with DyReLU-B pieces other than two: the 3x3 layers of D = 1 only (a 5x5 eval runs in the tile kernel,
+// conv_kernels.cu, and DyMN has no dilated layer)
+constexpr int kDyMinB = 2;
 template <typename T, int K, int S, int P, int MINB, int D = 1>
-int launch_mode(const SlideArgs& a, int mode, int xact_code, dim3 grid, size_t smem, cudaStream_t st) {
+int launch_mode(const SlideArgs& a, int mode, int xact_code, dim3 grid, size_t smem, cudaStream_t st, int dyk = 2) {
+  if (mode == 1 && dyk != 2 && a.dy.theta != nullptr) {
+    if constexpr (K == 3 && D == 1) {
+      // 2 DM coefficients per channel vector on top of the window: these instances run at kDyMinB CTAs per SM, where
+      // they keep everything in registers (no spills, DESIGN.md section 4)
+      switch (dyk) {
+        case 1: launch_one<T, K, S, P, 1, -1, kDyMinB, D, 1>(a, grid, smem, st); break;
+        case 3: launch_one<T, K, S, P, 1, -1, kDyMinB, D, 3>(a, grid, smem, st); break;
+        case 4: launch_one<T, K, S, P, 1, -1, kDyMinB, D, 4>(a, grid, smem, st); break;
+        default: eat_set_error("dw slide: DyReLU-B takes 1..4 linear pieces"); return EAT_ERR_UNSUPPORTED;
+      }
+      return EAT_OK;
+    }
+    eat_set_error("dw slide: DyReLU-B pieces other than two need a 3x3 undilated layer");
+    return EAT_ERR_UNSUPPORTED;
+  }
   if (mode == 1) launch_one<T, K, S, P, 1, -1, MINB, D>(a, grid, smem, st);
   else if (mode == 2) {
     if (S != 1) { eat_set_error("dw slide: data-gradient mode is stride 1 only"); return EAT_ERR_UNSUPPORTED; }
@@ -458,7 +490,7 @@ int launch_mode(const SlideArgs& a, int mode, int xact_code, dim3 grid, size_t s
 }
 
 template <typename T, int D = 1>
-int launch_slide(SlideArgs a, int B, int k, int stride, int mode, int xact_code, cudaStream_t st) {
+int launch_slide(SlideArgs a, int B, int k, int stride, int mode, int xact_code, cudaStream_t st, int dyk = 2) {
   constexpr int V = Vec<T>::N;
   constexpr bool kF32 = V == 4;
   const int cv = a.C / V;
@@ -478,8 +510,8 @@ int launch_slide(SlideArgs a, int B, int k, int stride, int mode, int xact_code,
     if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4, 2>(a, mode, xact_code, grid, smem, st);
     else if (k == 5 && stride == 1) rc = launch_mode<T, 5, 1, kF32 ? 2 : 1, 3, 2>(a, mode, xact_code, grid, smem, st);
     else { eat_set_error("dw slide: dilation 2 needs k in {3,5} and stride 1"); return EAT_ERR_UNSUPPORTED; }
-  } else if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4>(a, mode, xact_code, grid, smem, st);
-  else if (k == 3 && stride == 2) rc = launch_mode<T, 3, 2, kF32 ? 2 : 1, 5>(a, mode, xact_code, grid, smem, st);
+  } else if (k == 3 && stride == 1) rc = launch_mode<T, 3, 1, kF32 ? 4 : 2, 4>(a, mode, xact_code, grid, smem, st, dyk);
+  else if (k == 3 && stride == 2) rc = launch_mode<T, 3, 2, kF32 ? 2 : 1, 5>(a, mode, xact_code, grid, smem, st, dyk);
   else if (k == 5 && stride == 1) rc = launch_mode<T, 5, 1, kF32 ? 2 : 1, 3>(a, mode, xact_code, grid, smem, st);
   else if (k == 5 && stride == 2) rc = launch_mode<T, 5, 2, kF32 ? 2 : 1, 3>(a, mode, xact_code, grid, smem, st);
   else { eat_set_error("dw slide: only k in {3,5}, stride in {1,2}"); return EAT_ERR_UNSUPPORTED; }
@@ -1566,7 +1598,7 @@ namespace {
 // dil 2 (stride 1, padding 2 * (k-1)/2): the output has the input's size
 int slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
                  int dil, InXform xf, const float* scale, const float* shift, int act, const void* res, int flip,
-                 float* pool, double* ssum, double* ssq, cudaStream_t st, DyEpi dy) {
+                 float* pool, double* ssum, double* ssq, cudaStream_t st, DyEpi dy, int dyk = 2) {
   const int V = dtype == EAT_BF16 ? 8 : 4;
   if (C % V != 0) { eat_set_error("dw conv: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
   const int pad = (k - 1) / 2 * dil;
@@ -1585,8 +1617,8 @@ int slide_launch(const void* in, const float* wt, void* out, int dtype, int B, i
     if (dtype == EAT_BF16) return launch_slide<__nv_bfloat16, 2>(a, B, k, stride, mode, xact_code, st);
     return launch_slide<float, 2>(a, B, k, stride, mode, xact_code, st);
   }
-  if (dtype == EAT_BF16) return launch_slide<__nv_bfloat16>(a, B, k, stride, mode, xact_code, st);
-  return launch_slide<float>(a, B, k, stride, mode, xact_code, st);
+  if (dtype == EAT_BF16) return launch_slide<__nv_bfloat16>(a, B, k, stride, mode, xact_code, st, dyk);
+  return launch_slide<float>(a, B, k, stride, mode, xact_code, st, dyk);
 }
 
 int wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
@@ -1637,8 +1669,9 @@ int dil_check(const char* who, int dtype, int B, int F, int T, int C, int k, int
 
 int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B, int F, int Tn, int C, int k, int stride,
                     InXform xf, const float* scale, const float* shift, int act, const void* res, int flip, float* pool,
-                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy) {
-  return slide_launch(in, wt, out, dtype, B, F, Tn, C, k, stride, 1, xf, scale, shift, act, res, flip, pool, ssum, ssq, st, dy);
+                    double* ssum, double* ssq, cudaStream_t st, DyEpi dy, int dyk) {
+  return slide_launch(in, wt, out, dtype, B, F, Tn, C, k, stride, 1, xf, scale, shift, act, res, flip, pool, ssum, ssq, st, dy,
+                      dyk);
 }
 
 int dw_wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,

@@ -1,6 +1,8 @@
 // Small kernels of the DyMN context path (reference models/dymn/dy_block.py):
 //   ContextGen pooling (:236-237), sequence average pooling (:227-233,249), DynamicConv attention
 //   softmax(Linear(h_c)/T) (:104-107) and the per-sample depthwise weight mix (:111-117).
+#include <cstdio>
+
 #include "common.cuh"
 
 namespace {
@@ -263,6 +265,147 @@ __global__ void __launch_bounds__(256) dy_act_bwd_kernel(const T* __restrict__ d
   }
 }
 
+// ---- DyReLU-B with DM = 1, 3 or 4 linear pieces (dyrelu_k; theta [B, C, 2 DM] channel-major).  The kernels above are the
+// DM = 2 instances.  p = max_m (u a_m + b_m) * ca_f * ca_t (dy_block.py:179-188); DM = 1 is the affine map u a_0 + b_0.
+template <typename T, int DM>
+__global__ void __launch_bounds__(256) dy_act_fwd_m_kernel(const T* __restrict__ z, T* __restrict__ out, DyActCtx c,
+                                                           int Fo, int To, int C) {
+  const int b = blockIdx.y;
+  const int cv = C / 4;
+  const long long nvec = (long long)Fo * To * cv;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+    const int c0 = (int)(i % cv) * 4;
+    const long long pix = i / cv;
+    const int to = (int)(pix % To), fo = (int)(pix / To);
+    const size_t off = ((size_t)b * Fo * To + pix) * C + c0;
+    float v[4];
+    V4<T>::load(z + off, v);
+    const float4 f4 = *reinterpret_cast<const float4*>(c.ca_f + ((size_t)b * Fo + fo) * C + c0);
+    const float4 t4 = *reinterpret_cast<const float4*>(c.ca_t + ((size_t)b * To + to) * C + c0);
+    const float q[4] = {f4.x * t4.x, f4.y * t4.y, f4.z * t4.z, f4.w * t4.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      DyCoef<DM> co;
+      co.load(c.theta + ((size_t)b * C + c0 + k) * (2 * DM), c.lam, c.init);
+      v[k] = co.apply(fmaf(v[k], c.scale[c0 + k], c.shift[c0 + k])) * q[k];
+    }
+    V4<T>::store(out + off, v);
+  }
+}
+
+// Backward of the above, laid out as dy_act_bwd_kernel (s_coef holds 2 DM sums per channel).  Each pixel's gradient goes
+// to the piece that attains the max; on a tie, to the lowest piece index (the M = 2 kernel's `l1 >= l2` rule; the
+// reference's torch.max(dim=-1) also returns one index).
+template <typename T, int DM>
+__global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__ dp, const T* __restrict__ z, DyActCtx c,
+                                                           T* __restrict__ du, float* __restrict__ dcaf,
+                                                           float* __restrict__ dcat, float* __restrict__ dcoef, int Fo,
+                                                           int To, int C) {
+  constexpr int NC = 2 * DM;
+  extern __shared__ float smem[];
+  float* s_caf = smem;              // [Fo][32]
+  float* s_coef = smem + Fo * 32;   // [32][NC]
+  const int b = blockIdx.y;
+  const int chunks = ceil_div(C, 32);
+  const int chunk = blockIdx.x % chunks, tblk = blockIdx.x / chunks;
+  const int cvec = threadIdx.x & 7, tslot = threadIdx.x >> 3;
+  const int c0 = chunk * 32 + cvec * 4, to = tblk * 32 + tslot;
+  for (int i = threadIdx.x; i < Fo * 32 + 32 * NC; i += 256) smem[i] = 0.f;
+  __syncthreads();
+  const bool live = c0 < C && to < To;
+  DyCoef<DM> co[4];
+  float sc[4], sh[4], ct[4], g_ct[4], g_a[DM][4], g_b[DM][4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    co[k].zero();
+    sc[k] = sh[k] = ct[k] = g_ct[k] = 0.f;
+#pragma unroll
+    for (int m = 0; m < DM; ++m) g_a[m][k] = g_b[m][k] = 0.f;
+  }
+  if (live) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      co[k].load(c.theta + ((size_t)b * C + c0 + k) * NC, c.lam, c.init);
+      sc[k] = c.scale[c0 + k]; sh[k] = c.shift[c0 + k];
+    }
+    const float4 t4 = *reinterpret_cast<const float4*>(c.ca_t + ((size_t)b * To + to) * C + c0);
+    ct[0] = t4.x; ct[1] = t4.y; ct[2] = t4.z; ct[3] = t4.w;
+  }
+  for (int fo = 0; fo < Fo; ++fo) {
+    float dcf[4] = {0.f, 0.f, 0.f, 0.f};
+    if (live) {
+      const size_t off = (((size_t)b * Fo + fo) * To + to) * C + c0;
+      float g[4], zv[4], o[4];
+      V4<T>::load(dp + off, g);
+      V4<T>::load(z + off, zv);
+      const float4 f4 = *reinterpret_cast<const float4*>(c.ca_f + ((size_t)b * Fo + fo) * C + c0);
+      const float cf[4] = {f4.x, f4.y, f4.z, f4.w};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float u = fmaf(zv[k], sc[k], sh[k]);
+        float r = fmaf(u, co[k].a[0], co[k].b[0]), slope = co[k].a[0];
+        int arg = 0;
+#pragma unroll
+        for (int m = 1; m < DM; ++m) {
+          const float l = fmaf(u, co[k].a[m], co[k].b[m]);
+          if (l > r) { r = l; slope = co[k].a[m]; arg = m; }
+        }
+        const float dr = g[k] * cf[k] * ct[k];
+        dcf[k] = g[k] * r * ct[k];
+        g_ct[k] = fmaf(g[k] * r, cf[k], g_ct[k]);
+        o[k] = dr * slope;
+#pragma unroll
+        for (int m = 0; m < DM; ++m)
+          if (arg == m) { g_a[m][k] = fmaf(dr, u, g_a[m][k]); g_b[m][k] += dr; }
+      }
+      V4<T>::store(du + off, o);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      dcf[k] += __shfl_xor_sync(0xffffffffu, dcf[k], 8);
+      dcf[k] += __shfl_xor_sync(0xffffffffu, dcf[k], 16);
+    }
+    if ((threadIdx.x & 31) < 8) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) atomicAdd(&s_caf[fo * 32 + cvec * 4 + k], dcf[k]);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+#pragma unroll
+    for (int j = 0; j < NC; ++j) {
+      float v = j < DM ? g_a[j < DM ? j : 0][k] : g_b[j < DM ? 0 : j - DM][k];
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if ((threadIdx.x & 31) < 8) atomicAdd(&s_coef[(cvec * 4 + k) * NC + j], v);
+    }
+  }
+  if (live) {
+    float* dct = dcat + ((size_t)b * To + to) * C + c0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) dct[k] = g_ct[k];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < Fo * 32; i += 256) {
+    const int fo = i / 32, cc = chunk * 32 + (i & 31);
+    if (cc < C) atomicAdd(dcaf + ((size_t)b * Fo + fo) * C + cc, s_caf[i]);
+  }
+  if (threadIdx.x < 32 * NC) {
+    const int cc = chunk * 32 + threadIdx.x / NC;
+    if (cc < C) atomicAdd(dcoef + ((size_t)b * C + cc) * NC + threadIdx.x % NC, s_coef[threadIdx.x]);
+  }
+}
+
+// dpre[i] = dcoef[i] * lam[i % 2DM] * 2 s (1 - s), s = theta[i]: dyrelu_coef_bwd_kernel for DM pieces
+template <int DM>
+__global__ void dyrelu_coef_bwd_m_kernel(const float* __restrict__ dcoef, const float* __restrict__ theta,
+                                         const float* __restrict__ lam, float* __restrict__ dpre, long long n) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float s = theta[i];
+    dpre[i] = dcoef[i] * lam[i % (2 * DM)] * 2.f * s * (1.f - s);
+  }
+}
+
 // dpre[b,c,j] = dcoef[b,c,j] * lam[j] * 2 * s (1 - s),  s = theta[b,c,j]      (DyReLU coefficient net, dy_block.py:157-160,179)
 __global__ void dyrelu_coef_bwd_kernel(const float* __restrict__ dcoef, const float* __restrict__ theta,
                                        const float* __restrict__ lam, float* __restrict__ dpre, long long n) {
@@ -504,6 +647,93 @@ int eat_dy_act_bwd(const void* dp, const void* z, void* du, int dtype, const flo
 int eat_dyrelu_coef_bwd(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n, cudaStream_t st) {
   if (n == 0) return EAT_OK;
   dyrelu_coef_bwd_kernel<<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+// argument checks of the DyReLU-B entry points with M pieces, before any launch
+static int dym_check(const char* who, int dtype, int B, int Fo, int To, int C, int pieces, bool null_ptr) {
+  char msg[160];
+  int rc = EAT_OK;
+  if (pieces < 1 || pieces > 4) {
+    snprintf(msg, sizeof msg, "%s: DyReLU-B takes 1..4 linear pieces (got %d)", who, pieces);
+    rc = EAT_ERR_UNSUPPORTED;
+  } else if (dtype != EAT_F32 && dtype != EAT_BF16) { snprintf(msg, sizeof msg, "%s: dtype must be fp32 (0) or bf16 (1)", who); rc = EAT_ERR_ARG; }
+  else if (B < 0 || Fo < 1 || To < 1 || C < 1) { snprintf(msg, sizeof msg, "%s: B >= 0 and Fo, To, C >= 1 required", who); rc = EAT_ERR_ARG; }
+  else if (C % 4 != 0) { snprintf(msg, sizeof msg, "%s: channels must be a multiple of 4 (got %d)", who, C); rc = EAT_ERR_ARG; }
+  else if (null_ptr) { snprintf(msg, sizeof msg, "%s: every tensor pointer is required", who); rc = EAT_ERR_ARG; }
+  if (rc != EAT_OK) eat_set_error(msg);
+  return rc;
+}
+
+int eat_dy_act_fwd_m(const void* z, void* out, int dtype, const float* scale, const float* shift, const float* theta,
+                     const float* lam, const float* init, const float* ca_f, const float* ca_t, int pieces, int B, int Fo,
+                     int To, int C, cudaStream_t st) {
+  const bool null_ptr = !z || !out || !scale || !shift || !theta || !lam || !init || !ca_f || !ca_t;
+  if (int rc = dym_check("dy_act_fwd_m", dtype, B, Fo, To, C, pieces, null_ptr)) return rc;
+  if (B == 0) return EAT_OK;
+  if (pieces == 2) return eat_dy_act_fwd(z, out, dtype, scale, shift, theta, lam, init, ca_f, ca_t, B, Fo, To, C, st);
+  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
+  dim3 grid(max(1, min(kNumSMs * 8 / max(B, 1) + 1, (int)ceil_div_ll((long long)Fo * To * (C / 4), 256))), B);
+#define EAT_DYF(DM)                                                                                                      \
+  do {                                                                                                                   \
+    if (dtype == EAT_BF16) dy_act_fwd_m_kernel<__nv_bfloat16, DM><<<grid, 256, 0, st>>>((const __nv_bfloat16*)z, (__nv_bfloat16*)out, c, Fo, To, C); \
+    else dy_act_fwd_m_kernel<float, DM><<<grid, 256, 0, st>>>((const float*)z, (float*)out, c, Fo, To, C);            \
+  } while (0)
+  if (pieces == 1) EAT_DYF(1);
+  else if (pieces == 3) EAT_DYF(3);
+  else EAT_DYF(4);
+#undef EAT_DYF
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int eat_dy_act_bwd_m(const void* dp, const void* z, void* du, int dtype, const float* scale, const float* shift,
+                     const float* theta, const float* lam, const float* init, const float* ca_f, const float* ca_t,
+                     float* dcaf, float* dcat, float* dcoef, int pieces, int B, int Fo, int To, int C, cudaStream_t st) {
+  const bool null_ptr = !dp || !z || !du || !scale || !shift || !theta || !lam || !init || !ca_f || !ca_t || !dcaf ||
+                        !dcat || !dcoef;
+  if (int rc = dym_check("dy_act_bwd_m", dtype, B, Fo, To, C, pieces, null_ptr)) return rc;
+  if (B == 0) return EAT_OK;
+  if (pieces == 2)
+    return eat_dy_act_bwd(dp, z, du, dtype, scale, shift, theta, lam, init, ca_f, ca_t, dcaf, dcat, dcoef, B, Fo, To, C, st);
+  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
+  dim3 grid(ceil_div(C, 32) * ceil_div(To, 32), B);
+  const size_t smem = ((size_t)Fo * 32 + 32 * 2 * pieces) * sizeof(float);
+#define EAT_DYB(DM)                                                                                                      \
+  do {                                                                                                                   \
+    if (dtype == EAT_BF16)                                                                                               \
+      dy_act_bwd_m_kernel<__nv_bfloat16, DM><<<grid, 256, smem, st>>>((const __nv_bfloat16*)dp, (const __nv_bfloat16*)z, c, (__nv_bfloat16*)du, dcaf, dcat, dcoef, Fo, To, C); \
+    else                                                                                                                 \
+      dy_act_bwd_m_kernel<float, DM><<<grid, 256, smem, st>>>((const float*)dp, (const float*)z, c, (float*)du, dcaf, dcat, dcoef, Fo, To, C); \
+  } while (0)
+  if (pieces == 1) EAT_DYB(1);
+  else if (pieces == 3) EAT_DYB(3);
+  else EAT_DYB(4);
+#undef EAT_DYB
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int eat_dyrelu_coef_bwd_m(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n, int pieces,
+                          cudaStream_t st) {
+  char msg[128];
+  if (pieces < 1 || pieces > 4) {
+    snprintf(msg, sizeof msg, "dyrelu_coef_bwd_m: DyReLU-B takes 1..4 linear pieces (got %d)", pieces);
+    eat_set_error(msg);
+    return EAT_ERR_UNSUPPORTED;
+  }
+  if (n < 0 || n % (2 * pieces) != 0) {
+    snprintf(msg, sizeof msg, "dyrelu_coef_bwd_m: n must be a non-negative multiple of 2M = %d (got %lld)", 2 * pieces, n);
+    eat_set_error(msg);
+    return EAT_ERR_ARG;
+  }
+  if (!dcoef || !theta || !lam || !dpre) { eat_set_error("dyrelu_coef_bwd_m: every tensor pointer is required"); return EAT_ERR_ARG; }
+  if (n == 0) return EAT_OK;
+  if (pieces == 2) return eat_dyrelu_coef_bwd(dcoef, theta, lam, dpre, n, st);
+  if (pieces == 1) dyrelu_coef_bwd_m_kernel<1><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
+  else if (pieces == 3) dyrelu_coef_bwd_m_kernel<3><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
+  else dyrelu_coef_bwd_m_kernel<4><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }

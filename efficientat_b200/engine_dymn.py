@@ -163,13 +163,20 @@ class DyMNEngine(MNEngine):
         L.dyconv_mix_dw(m.depth_conv.weight.data_ptr(), att.data_ptr(), wt.data_ptr(), B, blk.cexp, blk.k,
                         m.depth_conv.k, st)
         coef = m.depth_act.coef_net[0]
-        theta = torch.empty(B, 4 * blk.cexp, device=dev, dtype=f32)
-        self._gemm(h_c, coef.weight, theta, B, 4 * blk.cexp, H, bias=coef.bias, act=SIG, a_code=0, c_code=0)
+        npc = m.depth_act.M                                 # DyReLU-B pieces: theta [B, C, 2M]
+        theta = torch.empty(B, 2 * npc * blk.cexp, device=dev, dtype=f32)
+        self._gemm(h_c, coef.weight, theta, B, 2 * npc * blk.cexp, H, bias=coef.bias, act=SIG, a_code=0, c_code=0)
         sc = self._fold(m.depth_norm, dev)
         d = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
-        L.dw_conv_fwd_dy(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
-                         0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), theta.data_ptr(), m.depth_act.lambdas.data_ptr(),
-                         m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(), 0, 0, st)
+        if npc == 2:
+            L.dw_conv_fwd_dy(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
+                             0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), theta.data_ptr(), m.depth_act.lambdas.data_ptr(),
+                             m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(), 0, 0, st)
+        else:
+            L.dw_conv_fwd_dy_m(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
+                               0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), theta.data_ptr(),
+                               m.depth_act.lambdas.data_ptr(), m.depth_act.init_v.data_ptr(), ca_f.data_ptr(),
+                               ca_t.data_ptr(), npc, 0, 0, st)
         # ---- project: DynamicConv 1x1 + BN (+ residual)
         att = attention(m.proj_conv)
         sc = self._fold(m.proj_norm, dev)
@@ -269,19 +276,28 @@ class DyMNEngine(MNEngine):
         L.dyconv_mix_dw(m.depth_conv.weight.data_ptr(), att_d.data_ptr(), wt.data_ptr(), B, blk.cexp, blk.k,
                         m.depth_conv.k, st)
         coef = m.depth_act.coef_net[0]
-        theta = torch.empty(B, 4 * blk.cexp, device=dev, dtype=f32)
-        self._gemm(h_c, coef.weight, theta, B, 4 * blk.cexp, H, bias=coef.bias, act=SIG, a_code=0, c_code=0)
+        npc = m.depth_act.M                                 # DyReLU-B pieces: theta [B, C, 2M]
+        theta = torch.empty(B, 2 * npc * blk.cexp, device=dev, dtype=f32)
+        self._gemm(h_c, coef.weight, theta, B, 2 * npc * blk.cexp, H, bias=coef.bias, act=SIG, a_code=0, c_code=0)
         Mo = B * Fo * To
         z2 = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         stt = self._new_stats(blk.cexp, dev)
-        L.dw_conv_fwd_dy(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
-                         _ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
-                         blk.act if dw_sc is not None else 0, 0, 0, 0, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+        xs = (_ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
+              blk.act if dw_sc is not None else 0)
+        if npc == 2:
+            L.dw_conv_fwd_dy(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
+                             s, *xs, 0, 0, 0, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+        else:
+            L.dw_conv_fwd_dy_m(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp,
+                               blk.k, s, *xs, 0, 0, 0, 0, 0, 0, 0, npc, stt[0].data_ptr(), stt[1].data_ptr(), st)
         sc2, sv2 = self._finalize(m.depth_norm, stt, Mo, dev)
         p = torch.empty_like(z2)
-        L.dy_act_fwd(z2.data_ptr(), p.data_ptr(), dc, sc2[0].data_ptr(), sc2[1].data_ptr(), theta.data_ptr(),
-                     m.depth_act.lambdas.data_ptr(), m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(),
-                     B, Fo, To, blk.cexp, st)
+        act_args = (z2.data_ptr(), p.data_ptr(), dc, sc2[0].data_ptr(), sc2[1].data_ptr(), theta.data_ptr(),
+                    m.depth_act.lambdas.data_ptr(), m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr())
+        if npc == 2:
+            L.dy_act_fwd(*act_args, B, Fo, To, blk.cexp, st)
+        else:
+            L.dy_act_fwd_m(*act_args, npc, B, Fo, To, blk.cexp, st)
         att_p = attention(m.proj_conv)
         z3 = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
         stt = self._new_stats(blk.cout, dev)
@@ -378,19 +394,29 @@ class DyMNEngine(MNEngine):
         # ---- CoordAtt * DyReLU-B * BN2 backward
         dcaf = torch.zeros(B, Fo, C, device=dev, dtype=f32)
         dcat = torch.empty(B, To, C, device=dev, dtype=f32)
-        dcoef = torch.zeros(B, C, 4, device=dev, dtype=f32)
-        du = torch.empty_like(R["z2"])
         act_mod = m.depth_act
-        L.dy_act_bwd(dp.data_ptr(), R["z2"].data_ptr(), du.data_ptr(), dc, R["sc2"][0].data_ptr(), R["sc2"][1].data_ptr(),
-                     R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), act_mod.init_v.data_ptr(), R["ca_f"].data_ptr(),
-                     R["ca_t"].data_ptr(), dcaf.data_ptr(), dcat.data_ptr(), dcoef.data_ptr(), B, Fo, To, C, st)
+        npc = act_mod.M                                     # DyReLU-B pieces: dcoef [B, C, 2M]
+        dcoef = torch.zeros(B, C, 2 * npc, device=dev, dtype=f32)
+        du = torch.empty_like(R["z2"])
+        act_args = (dp.data_ptr(), R["z2"].data_ptr(), du.data_ptr(), dc, R["sc2"][0].data_ptr(), R["sc2"][1].data_ptr(),
+                    R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), act_mod.init_v.data_ptr(), R["ca_f"].data_ptr(),
+                    R["ca_t"].data_ptr(), dcaf.data_ptr(), dcat.data_ptr(), dcoef.data_ptr())
+        if npc == 2:
+            L.dy_act_bwd(*act_args, B, Fo, To, C, st)
+        else:
+            L.dy_act_bwd_m(*act_args, npc, B, Fo, To, C, st)
         # DyReLU coefficient net
         coef = act_mod.coef_net[0]
-        dpre = torch.empty(B, 4 * C, device=dev, dtype=f32)
-        L.dyrelu_coef_bwd(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(), B * 4 * C, st)
-        self._wgrad(dpre, h_c, G[coef.weight], G[coef.bias], B, 4 * C, H, g_code=0, a_code=0)
+        nco = 2 * npc * C
+        dpre = torch.empty(B, nco, device=dev, dtype=f32)
+        if npc == 2:
+            L.dyrelu_coef_bwd(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(), B * nco, st)
+        else:
+            L.dyrelu_coef_bwd_m(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(),
+                                B * nco, npc, st)
+        self._wgrad(dpre, h_c, G[coef.weight], G[coef.bias], B, nco, H, g_code=0, a_code=0)
         dh_new = torch.empty_like(dh_c)
-        self._gemm(dpre, coef.weight, dh_new, B, H, 4 * C, a_code=0, c_code=0, w_trans=True, res=dh_c)
+        self._gemm(dpre, coef.weight, dh_new, B, H, nco, a_code=0, c_code=0, w_trans=True, res=dh_c)
         dh_c = dh_new
         # coordinate-attention nets (conv_f / conv_t are Linear layers over the context dimension)
         dhcat = torch.empty(B, P, H, device=dev, dtype=f32)

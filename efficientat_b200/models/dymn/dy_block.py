@@ -83,12 +83,18 @@ class DyReLU(FusedOnly):
 
 
 class DyReLUB(DyReLU):
-    """max(a1 x + b1, a2 x + b2) with per-(sample, channel) coefficients (dy_block.py:165-188)."""
+    """max_m (a_m x + b_m) over M linear pieces with per-(sample, channel) coefficients (dy_block.py:165-188).
+    M = dyrelu_k in 1..4: the kernels hold the 2M coefficients of a channel in registers, and four pieces is where
+    that budget ends.  On a tie the gradient goes to the lowest piece index (for M = 2 the reference's torch.maximum
+    splits it in half; for M != 2 its torch.max also picks one piece)."""
+
+    MAX_PIECES = 4
 
     def __init__(self, channels, context_dim, M=2):
+        if not 1 <= M <= self.MAX_PIECES:
+            raise NotImplementedError(f"DyReLUB: dyrelu_k (the number of linear pieces M) must be in "
+                                      f"1..{self.MAX_PIECES} for the fused engine, got {M}")
         super().__init__(channels, context_dim, M)
-        if M != 2:
-            raise NotImplementedError("DyReLUB: only dyrelu_k == 2 is implemented by the fused engine")
         self.coef_net[-1] = nn.Linear(context_dim, 2 * M * self.channels)
 
 

@@ -173,6 +173,18 @@ int eat_dw_conv_fwd_dy(const void* in, const float* wt, long long wt_bstride, vo
                        const float* scale, const float* shift, const float* theta, const float* lam,
                        const float* init, const float* ca_f, const float* ca_t, double* stat_sum, double* stat_sq,
                        cudaStream_t stream);
+/* eat_dw_conv_fwd_dy with M = `pieces` DyReLU-B linear pieces, 1..4 (dy_block.py:142-188, dyrelu_k):
+ * theta [B, C, 2M] channel-major, lam / init [2M]; out = max_m (a_m u + b_m) * ca_f * ca_t with
+ * a_m = (2 theta[m] - 1) lam[m] + init[m], b_m = (2 theta[M+m] - 1) lam[M+m] + init[M+m], u = BN(conv).  The training
+ * form (in_scale/in_shift, stat_sum/stat_sq, no theta) does not depend on M.  Before any launch: pieces outside 1..4,
+ * k outside {3,5}, stride outside {1,2} -> EAT_ERR_UNSUPPORTED; bad dtype or sizes, C not a multiple of the vector
+ * width (4 fp32, 8 bf16), pointers that come in sets given partly, the training transform or statistics together with
+ * the eval epilogue -> EAT_ERR_ARG.  B = 0 is a no-op. */
+int eat_dw_conv_fwd_dy_m(const void* in, const float* wt, long long wt_bstride, void* out, int dtype, int B, int F, int T,
+                         int C, int k, int stride, const float* in_scale, const float* in_shift, int in_act,
+                         const float* scale, const float* shift, const float* theta, const float* lam,
+                         const float* init, const float* ca_f, const float* ca_t, int pieces, double* stat_sum,
+                         double* stat_sq, cudaStream_t stream);
 /* ContextGen pooling (dy_block.py:236-240): out [B, F+T, C] fp32 = [mean over T | mean over F]. */
 int eat_ctx_pool(const void* x, int dtype, float* out, int B, int F, int T, int C, cudaStream_t stream);
 /* Sequence pooling of ContextGen (dy_block.py:227-233,249): AvgPool(3, stride, pad 1) or copy (stride 1) of rows
@@ -197,6 +209,19 @@ int eat_dy_act_bwd(const void* dp, const void* z, void* du, int dtype, const flo
 /* dpre = dcoef * lam * 2 s (1-s) with s = theta (DyReLU coefficient net); out = g * s * (1-s) (sigmoid backward). */
 int eat_dyrelu_coef_bwd(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n,
                         cudaStream_t stream);
+/* The three above with M = `pieces` DyReLU-B linear pieces, 1..4: theta [B, C, 2M], lam / init [2M], dcoef [B, C, 2M]
+ * (accumulated; da_m = sum du x [m = argmax], db_m = sum du [m = argmax]).  The pixel's gradient goes to the one piece
+ * that attains the max; on a tie, to the lowest piece index (M = 2 included).  n = B * C * 2M.  Before any launch: pieces
+ * outside 1..4 -> EAT_ERR_UNSUPPORTED; bad dtype or sizes, C not a multiple of 4, n not a multiple of 2M, a null
+ * pointer -> EAT_ERR_ARG.  B = 0 (n = 0) is a no-op. */
+int eat_dy_act_fwd_m(const void* z, void* out, int dtype, const float* scale, const float* shift, const float* theta,
+                     const float* lam, const float* init, const float* ca_f, const float* ca_t, int pieces, int B, int Fo,
+                     int To, int C, cudaStream_t stream);
+int eat_dy_act_bwd_m(const void* dp, const void* z, void* du, int dtype, const float* scale, const float* shift,
+                     const float* theta, const float* lam, const float* init, const float* ca_f, const float* ca_t,
+                     float* dcaf, float* dcat, float* dcoef, int pieces, int B, int Fo, int To, int C, cudaStream_t stream);
+int eat_dyrelu_coef_bwd_m(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n, int pieces,
+                          cudaStream_t stream);
 int eat_sigmoid_bwd(const float* g, const float* s, float* out, long long n, cudaStream_t stream);
 /* softmax(Linear(h_c)/T) backward: dWr/dbr accumulated, dh_c[b,:] += dlogit . Wr.  k in 1..4, as eat_dyconv_att. */
 int eat_dyconv_att_bwd(const float* datt, const float* att, float temperature, const float* hc, const float* wr,
