@@ -142,6 +142,11 @@ int dw_slide_launch(const void* in, const float* wt, void* out, int dtype, int B
 int dw_wgrad_slide_launch(const void* dz, const void* in, InXform xf, float* dw, long long dw_bstride, int dtype, int B,
                           int F, int Tn, int C, int k, int stride, cudaStream_t st);
 
+// launch plan of the shared-memory tile kernel dw_tile_kernel (conv_kernels.cu): 32-channel chunks, FR x TT output tiles
+// per chunk, `groups` CTAs per (chunk, sample) that stride over the tiles; gridDim = (chunks * groups, B)
+struct DwTilePlan { int chunks, tiles, groups, FR, TT; };
+DwTilePlan dw_tile_plan(int B, int Fo, int To, int C, int stride);
+
 // z != nullptr: BatchNorm-backward reduce of the layer behind din in the epilogue (fp32 storage; see Dg2Args in dw_slide.cu)
 int dw_dgrad2_slide_launch(const void* dz, const float* wt, long long wt_bstride, const void* res, void* din, int dtype,
                            int B, int F, int Tn, int C, int k, cudaStream_t st, const void* z = nullptr,

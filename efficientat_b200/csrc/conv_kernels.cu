@@ -616,6 +616,22 @@ inline int grid_for(long long items, int per_block, int max_blocks = kNumSMs * 1
   return (int)g;
 }
 
+}  // namespace
+
+// about six CTAs per SM over all chunks and samples, never more CTAs per chunk than it has tiles
+DwTilePlan dw_tile_plan(int B, int Fo, int To, int C, int stride) {
+  DwTilePlan pl;
+  pl.FR = stride == 1 ? 8 : 4;
+  pl.TT = stride == 1 ? 32 : 16;
+  pl.chunks = ceil_div(C, 32);
+  pl.tiles = ceil_div(Fo, pl.FR) * ceil_div(To, pl.TT);
+  pl.groups = max(1, (kNumSMs * 6) / max(B * pl.chunks, 1));
+  if (pl.groups > pl.tiles) pl.groups = pl.tiles;
+  return pl;
+}
+
+namespace {
+
 template <typename T>
 int launch_dw(const T* in, const float* wt, T* out, int B, int F, int Tn, int C, int k, int stride, InXform xf,
               const float* scale, const float* shift, int act, const T* res, int flip, float* pool, double* ssum,
@@ -636,13 +652,9 @@ int launch_dw(const T* in, const float* wt, T* out, int B, int F, int Tn, int C,
                            pool, ssum, ssq, st, dy, dyk);
   if (k != 5) { eat_set_error("dw conv: only k in {3,5}, stride in {1,2}"); return EAT_ERR_UNSUPPORTED; }
   // shared-memory tiled kernel: grid.x = channel chunks x tile groups (each CTA strides over its group's tiles)
-  const int FR = stride == 1 ? 8 : 4, TT = stride == 1 ? 32 : 16;
-  const int IR = (FR - 1) * stride + k, IT = (TT - 1) * stride + k;
-  const int chunks = ceil_div(C, 32);
-  const int tiles = ceil_div(Fo, FR) * ceil_div(To, TT);
-  int groups = max(1, (kNumSMs * 6) / max(B * chunks, 1));
-  if (groups > tiles) groups = tiles;
-  dim3 grid(chunks * groups, B);
+  const DwTilePlan pl = dw_tile_plan(B, Fo, To, C, stride);
+  const int IR = (pl.FR - 1) * stride + k, IT = (pl.TT - 1) * stride + k;
+  dim3 grid(pl.chunks * pl.groups, B);
   size_t smem = ((size_t)IR * IT * 32 + (size_t)k * k * 32 + 64) * sizeof(float);
   const int tmode = (scale != nullptr || pool != nullptr || dy.theta != nullptr || dy.ca_f != nullptr) ? 1 : ((flip || res != nullptr) ? 2 : 0);
 #define EAT_DWM(KK, SS, MM, DK)                                                                                 \

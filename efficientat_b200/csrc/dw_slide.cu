@@ -137,6 +137,17 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
   const bool need_red = (kPool && a.pool != nullptr) || (kStats && a.stat_sum != nullptr);
   const int ppb = kST / ncv;
   const int cvl = tid % ncv, slot = tid / ncv;
+  // batch statistics as shifted sums: a thread sums d = o - K and d^2 in fp32, and the CTA combines
+  // sum o = sum d + n K, sum o^2 = sum d^2 + 2 K sum d + n K^2 in fp64.  K is the thread's first output whose window lies
+  // inside the image (until one comes, its first output): a border output, missing taps, can sit several std from the
+  // mean.  A thread sums thousands of outputs at the bench's batch; unshifted fp32 sums of o^2 lost the variance
+  // E[o^2] - E[o]^2 to cancellation when the mean is large against the std (~10x further from fp64 than PyTorch's fp32
+  // BatchNorm, tests/test_gpu_zz_dw_steady.py)
+  float lsum[V], lsq[V], kshift[V];
+  int nsum = 0;                                // outputs this thread has summed per channel
+  bool kinner = false;                         // K is an interior output
+#pragma unroll
+  for (int i = 0; i < V; ++i) { lsum[i] = 0.f; lsq[i] = 0.f; kshift[i] = 0.f; }
   if (slot < ppb) {
     const int c0 = (cv0 + cvl) * V;
     const float* wl = s_w + cvl * V;
@@ -169,9 +180,6 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
         for (int i = 0; i < V; ++i) dyc[i].load(a.dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), a.dy.lam, a.dy.init);
       }
     }
-    float lsum[V], lsq[V];
-#pragma unroll
-    for (int i = 0; i < V; ++i) { lsum[i] = 0.f; lsq[i] = 0.f; }
     int bb = b;                                  // sample of the current unit
     const T* inb = nullptr;
     T* outb = nullptr;
@@ -193,8 +201,25 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
 #pragma unroll
             for (int i = 0; i < V; ++i) { o[p][i] = act_fwd(fmaf(o[p][i], osc[i], osh[i]), a.act); lsum[i] += o[p][i]; }
           } else if (kStats) {
+            const int Fi = D == 1 ? F : Fs, Ti = D == 1 ? Tn : Ts;
+            const bool inner = fo * S >= PAD && fo * S - PAD + K <= Fi && to * S >= PAD && to * S - PAD + K <= Ti;
+            if (nsum == 0 || (inner && !kinner)) {   // re-base the sums so far onto this output
+              kinner = inner;
 #pragma unroll
-            for (int i = 0; i < V; ++i) { lsum[i] += o[p][i]; lsq[i] = fmaf(o[p][i], o[p][i], lsq[i]); }
+              for (int i = 0; i < V; ++i) {
+                const float dk = o[p][i] - kshift[i];
+                lsq[i] = fmaf((float)nsum * dk, dk, fmaf(-2.f * dk, lsum[i], lsq[i]));
+                lsum[i] = fmaf(-(float)nsum, dk, lsum[i]);
+                kshift[i] = o[p][i];
+              }
+            }
+#pragma unroll
+            for (int i = 0; i < V; ++i) {
+              const float d = o[p][i] - kshift[i];
+              lsum[i] += d;
+              lsq[i] = fmaf(d, d, lsq[i]);
+            }
+            ++nsum;
           }
           if (kDy && a.dy.theta != nullptr) {
             if constexpr (DM == 2) {
@@ -374,22 +399,32 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
         if (S == 2 && n + 1 < steps) feed(i0 + 2 * n + 1, Ph1{});   // the last odd row only feeds rows past the segment
       }
     }
-    if (need_red) {
+    if (kPool && need_red) {
 #pragma unroll
       for (int i = 0; i < V; ++i) atomicAdd(&s_sum[cvl * V + i], lsum[i]);
-      if (kStats) {
-#pragma unroll
-        for (int i = 0; i < V; ++i) atomicAdd(&s_sq[cvl * V + i], lsq[i]);
-      }
     }
   }
-  if (need_red) {
+  if (kPool && need_red) {
     __syncthreads();
-    for (int c = tid; c < cc; c += kST) {
-      const int cg = cv0 * V + c;
-      if (kPool && a.pool != nullptr) atomicAdd(a.pool + (size_t)b * C + cg, s_sum[c]);
-      if (kStats && a.stat_sum != nullptr) { atomicAdd(a.stat_sum + cg, (double)s_sum[c]); atomicAdd(a.stat_sq + cg, (double)s_sq[c]); }
+    for (int c = tid; c < cc; c += kST) atomicAdd(a.pool + (size_t)b * C + cv0 * V + c, s_sum[c]);
+  }
+  if (kStats && need_red) {
+    // every thread has finished its walk, so the weight table's shared memory takes the fp64 partials
+    double* d_sum = reinterpret_cast<double*>(smem);
+    double* d_sq = d_sum + cc;
+    __syncthreads();
+    for (int c = tid; c < 2 * cc; c += kST) d_sum[c] = 0.0;
+    __syncthreads();
+    if (slot < ppb) {
+#pragma unroll
+      for (int i = 0; i < V; ++i) {
+        const double k = kshift[i], sd = lsum[i];
+        atomicAdd(&d_sum[cvl * V + i], sd + nsum * k);
+        atomicAdd(&d_sq[cvl * V + i], (double)lsq[i] + k * (2.0 * sd + nsum * k));
+      }
     }
+    __syncthreads();
+    for (int c = tid; c < cc; c += kST) { atomicAdd(a.stat_sum + cv0 * V + c, d_sum[c]); atomicAdd(a.stat_sq + cv0 * V + c, d_sq[c]); }
   }
 }
 
@@ -436,11 +471,19 @@ inline SlidePlan plan_slide(int B, int Fo, int To, int cv, int V, int P, int S, 
   return pl;
 }
 
+// prefetch-ring depth of dw_slide_kernel: rows of NIN 16-byte vectors per thread next to the (k*k + 2) x cvc*V float
+// tables, three rows for chunks of <= 32 channels, two otherwise (eat_dw_ring_depth reports it)
+inline int slide_ring_depth(int K, int S, int P, int minb, int cvc, int V) {
+  const size_t smem = ((size_t)K * K + 2) * cvc * V * sizeof(float);
+  const size_t slot = (size_t)((P - 1) * S + K) * kST * 16;
+  return ring_depth((size_t)(227 * 1024) / minb - 1024, smem, slot, cvc * V <= 32 ? 3 : 2);
+}
+
 template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, int D = 1, int DM = 2>
 void launch_one(SlideArgs a, dim3 grid, size_t smem, cudaStream_t st) {
   constexpr int NIN = (P - 1) * S + K;
   const size_t slot = (size_t)NIN * kST * 16;
-  a.depth = ring_depth((size_t)(227 * 1024) / MINB - 1024, smem, slot, a.cvc * Vec<T>::N <= 32 ? 3 : 2);
+  a.depth = slide_ring_depth(K, S, P, MINB, a.cvc, Vec<T>::N);
   static unsigned long long mask0 = 0, mask1 = 0;
   if (a.depth > 0) {
     auto kern = dw_slide_kernel<T, K, S, P, MODE, XACT, MINB, true, D, DM>;
@@ -1759,6 +1802,12 @@ extern "C" int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int 
   const bool f32 = dtype != EAT_BF16;
   const int pad = (k - 1) / 2;
   const int Fo = (F + 2 * pad - k) / stride + 1, To = (T + 2 * pad - k) / stride + 1;
+  if (kind == 4) {                                   // dw_tile_kernel (conv_kernels.cu): 5x5 only, blockIdx.y is the sample
+    if (k != 5) { eat_set_error("dw_plan: kind 4 is the 5x5 tile kernel"); return EAT_ERR_ARG; }
+    const DwTilePlan pl = dw_tile_plan(B, Fo, To, C, stride);
+    plan[0] = pl.chunks; plan[1] = 32; plan[2] = pl.tiles; plan[3] = pl.groups; plan[4] = B; plan[5] = pl.FR;
+    return EAT_OK;
+  }
   int V = V0, P, minb, rows, cols, S = stride, Kp = k;
   if (kind == 0) {                                   // launch_slide
     P = (k == 3 && stride == 1) ? (f32 ? 4 : 2) : (f32 ? 2 : 1);
@@ -1775,10 +1824,26 @@ extern "C" int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int 
     P = 4; minb = k == 3 ? 4 : 3;
     rows = (F + 1) / 2; cols = T; S = 1; Kp = (k + 1) / 2;
   } else {
-    eat_set_error("dw_plan: kind must be 0, 1, 2 or 3");
+    eat_set_error("dw_plan: kind must be 0, 1, 2, 3 or 4");
     return EAT_ERR_ARG;
   }
   const SlidePlan pl = plan_slide(B, rows, cols, C / V, V, P, S, Kp, minb, per_sample != 0);
   plan[0] = pl.chunks; plan[1] = pl.cvc; plan[2] = pl.seg_rows; plan[3] = pl.groups; plan[4] = pl.gy; plan[5] = P;
+  return EAT_OK;
+}
+
+extern "C" int eat_dw_ring_depth(int dtype, int C, int k, int stride, int* depth) {
+  const int V = dtype == EAT_BF16 ? 8 : 4;
+  if (depth == nullptr || (dtype != EAT_F32 && dtype != EAT_BF16) || C < V || C % V != 0 || (k != 3 && k != 5) ||
+      (stride != 1 && stride != 2)) {
+    eat_set_error("dw_ring_depth: invalid arguments");
+    return EAT_ERR_ARG;
+  }
+  // as launch_slide: strip width and CTAs per SM of the undilated kernel, channel chunks of plan_slide
+  const bool f32 = dtype == EAT_F32;
+  const int P = (k == 3 && stride == 1) ? (f32 ? 4 : 2) : (f32 ? 2 : 1);
+  const int minb = k == 3 ? (stride == 1 ? 4 : 5) : 3;
+  const SlidePlan pl = plan_slide(1, 1, 1, C / V, V, P, stride, k, minb, false);
+  *depth = slide_ring_depth(k, stride, P, minb, pl.cvc, V);
   return EAT_OK;
 }

@@ -51,9 +51,16 @@ int eat_abi_version(void);
  * channel vectors are 4 channels for 3x3 and 2 for 5x5).  per_sample != 0: blockIdx.y must be the sample
  * (squeeze-excitation pooling, DynamicConv per-sample weights; ignored by kind 3).  plan[6] = {channel chunks, channel
  * vectors per chunk, output rows (row pairs for kind 2; din rows, or row pairs for stride 2, for kind 3) per segment,
- * CTA groups per chunk, gridDim.y, strip width}.  Exposed so the
+ * CTA groups per chunk, gridDim.y, strip width}.
+ * kind 4: the shared-memory tile kernel (csrc/conv_kernels.cu: the 5x5 eval forward and the 5x5 stride-1 data gradient
+ * above 256 channels; k must be 5, per_sample is ignored since blockIdx.y is always the sample).  plan[6] = {channel
+ * chunks, 32 channels per chunk, output tiles of FR x (32 / stride) pixels per chunk and sample, CTA groups per chunk
+ * (each CTA strides over tiles / groups of them), gridDim.y = B, FR}.  Exposed so the
  * host logic is testable without a device (tests/test_cabi.py). */
 int eat_dw_plan(int kind, int dtype, int B, int F, int T, int C, int k, int stride, int per_sample, int* plan);
+/* Host-only: the cp.async prefetch-ring depth in input rows (0: ring off) that the sliding-window kernel of
+ * eat_dw_conv_fwd / the stride-1 eat_dw_conv_dgrad takes for C channels, k x k, stride; EAT_DW_RING overrides it. */
+int eat_dw_ring_depth(int dtype, int C, int k, int stride, int* depth);
 int eat_device_check(int device);
 
 /* Fused log-mel front end.  Replaces AugmentMelSTFT.forward, models/preprocess.py:40-67

@@ -81,6 +81,22 @@ def test_depthwise_launch_plan_host_logic():
                             assert rounds * slots <= 1.34 * units, (kind, dtype, (F, T, C, k, s), list(plan), rounds * slots / units)
     with pytest.raises(RuntimeError):
         L.dw_plan(0, 0, 1, 8, 8, 6, 3, 1, 0, ctypes.addressof(plan))       # channels not a multiple of the vector width
+    # kind 4, the 5x5 tile kernel: 32-channel chunks, FR x 32/stride tiles, about six CTAs per SM over chunks and
+    # samples, never more CTAs per chunk than tiles; blockIdx.y is the sample
+    for B in (1, 3, 256):
+        for (F, T, C, k, s) in shapes:
+            if k != 5:
+                with pytest.raises(RuntimeError):
+                    L.dw_plan(4, 0, B, F, T, C, k, s, 0, ctypes.addressof(plan))
+                continue
+            L.dw_plan(4, 0, B, F, T, C, k, s, 0, ctypes.addressof(plan))
+            chunks, cc, tiles, groups, gy, FR = list(plan)
+            Fo, To = (F + 4 - k) // s + 1, (T + 4 - k) // s + 1
+            assert cc == 32 and chunks * 32 >= C > (chunks - 1) * 32 and gy == B and FR == (8 if s == 1 else 4)
+            assert tiles == -(-Fo // FR) * -(-To // (32 // s)) and 1 <= groups <= tiles
+            assert groups in (1, tiles) or chunks * groups * B <= 132 * 6
+            if B == 256 and tiles > 1:
+                assert groups < tiles                                     # several tiles per CTA at the bench batch
 
 
 def test_argument_errors_are_reported_before_any_launch():
