@@ -734,6 +734,50 @@ __global__ void __launch_bounds__(kThreads) stem_wgrad_kernel(const T* __restric
   }
 }
 
+// stem data gradient: dx[b,f,t] = sum_{c,ky,kx} w[c,ky,kx] * dz[b,fo,to,c] over the taps with f = fo*S-1+ky,
+// t = to*S-1+kx, where dz = scale * (dy * act'(z*scale+shift) - c1 - xhat*c2) is formed on load (eat_bn_bwd_apply's
+// formula; c1 = c2 = 0 for BatchNorm on running statistics).  One thread per input pixel, all channels in a fixed order:
+// no atomics, so the result is bitwise repeatable.  Lanes of a warp walk the same channel, so the weight and BatchNorm
+// loads are broadcasts.
+template <typename T, int S>
+__global__ void __launch_bounds__(kThreads) stem_dgrad_kernel(const T* __restrict__ dy, const T* __restrict__ z, BnCtx bn,
+                                                              const float* __restrict__ c1, const float* __restrict__ c2,
+                                                              const float* __restrict__ w, float* __restrict__ dx, int B,
+                                                              int F, int Tn, int C) {
+  constexpr int V = Vec<T>::N;
+  const int Fo = (F - 1) / S + 1, To = (Tn - 1) / S + 1;
+  const long long npix = (long long)B * F * Tn;
+  for (long long pix = (long long)blockIdx.x * kThreads + threadIdx.x; pix < npix; pix += (long long)gridDim.x * kThreads) {
+    const int t = (int)(pix % Tn), f = (int)((pix / Tn) % F), b = (int)(pix / ((long long)Tn * F));
+    float acc = 0.f;
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky) {
+      const int fs = f + 1 - ky;
+      if (fs < 0 || fs % S != 0 || fs / S >= Fo) continue;
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const int ts = t + 1 - kx;
+        if (ts < 0 || ts % S != 0 || ts / S >= To) continue;
+        const size_t base = (((size_t)b * Fo + fs / S) * To + ts / S) * C;
+        for (int c0 = 0; c0 < C; c0 += V) {
+          float g[V], zv[V];
+          Vec<T>::load(dy + base + c0, g);
+          Vec<T>::load(z + base + c0, zv);
+#pragma unroll
+          for (int k = 0; k < V; ++k) {
+            const int c = c0 + k;
+            const float sc = __ldg(bn.scale + c);
+            const float d = g[k] * act_bwd(fmaf(zv[k], sc, __ldg(bn.shift + c)), bn.act);
+            const float xhat = (zv[k] - __ldg(bn.mean + c)) * __ldg(bn.invstd + c);
+            acc = fmaf(__ldg(w + c * 9 + ky * 3 + kx), sc * (d - __ldg(c1 + c) - xhat * __ldg(c2 + c)), acc);
+          }
+        }
+      }
+    }
+    dx[pix] = acc;
+  }
+}
+
 // Row-oriented stem weight gradient (fp32 dz, C <= 64): same walk as stem_row_kernel; the U = 4 gradient vectors and
 // the 36 input values of a trip are requested before the first use (the pixel-at-a-time kernel above has ONE 16-byte
 // load in flight per thread).  APPLY: `dz` is the gradient dy at the BatchNorm + activation's output and dz is computed
@@ -1111,6 +1155,33 @@ int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, 
     stem_wgrad_kernel<__nv_bfloat16><<<grid, kThreads, smem, st>>>((const __nv_bfloat16*)dz, x, dw, B, F, T, Fo, To, C, stride);
   else
     stem_wgrad_kernel<float><<<grid, kThreads, smem, st>>>((const float*)dz, x, dw, B, F, T, Fo, To, C, stride);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int eat_stem_dgrad(const void* dy, int dtype, const void* z, const float* scale, const float* shift, const float* mean,
+                   const float* invstd, int act, const float* c1, const float* c2, const float* w, float* dx, int B, int F,
+                   int T, int C, int stride, cudaStream_t st) {
+  if (dtype != EAT_F32 && dtype != EAT_BF16) { eat_set_error("stem dgrad: dtype must be EAT_F32 or EAT_BF16"); return EAT_ERR_ARG; }
+  const int V = dtype == EAT_BF16 ? 8 : 4;
+  if (C < V || C % V != 0 || C / V > kThreads) { eat_set_error("stem dgrad: unsupported channel count"); return EAT_ERR_ARG; }
+  if (stride != 1 && stride != 2) { eat_set_error("stem dgrad: stride must be 1 or 2"); return EAT_ERR_UNSUPPORTED; }
+  if (act != EAT_ACT_NONE && act != EAT_ACT_RELU && act != EAT_ACT_HSWISH) {
+    eat_set_error("stem dgrad: act must be none, relu or hardswish"); return EAT_ERR_ARG;
+  }
+  if (B < 0 || F < 1 || T < 1) { eat_set_error("stem dgrad: bad sizes"); return EAT_ERR_ARG; }
+  if (B == 0) return EAT_OK;
+  if (dy == nullptr || z == nullptr || scale == nullptr || shift == nullptr || mean == nullptr || invstd == nullptr ||
+      c1 == nullptr || c2 == nullptr || w == nullptr || dx == nullptr) {
+    eat_set_error("stem dgrad: dy, z, scale, shift, mean, invstd, c1, c2, w and dx are required"); return EAT_ERR_ARG;
+  }
+  const long long npix = (long long)B * F * T;
+  const int grid = (int)min((long long)kNumSMs * 16, ceil_div_ll(npix, kThreads));
+  const BnCtx bn{scale, shift, mean, invstd, act};
+#define EAT_STEM_DG(TT, S_) stem_dgrad_kernel<TT, S_><<<grid, kThreads, 0, st>>>((const TT*)dy, (const TT*)z, bn, c1, c2, w, dx, B, F, T, C)
+  if (dtype == EAT_BF16) { if (stride == 2) EAT_STEM_DG(__nv_bfloat16, 2); else EAT_STEM_DG(__nv_bfloat16, 1); }
+  else { if (stride == 2) EAT_STEM_DG(float, 2); else EAT_STEM_DG(float, 1); }
+#undef EAT_STEM_DG
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }

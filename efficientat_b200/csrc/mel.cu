@@ -23,6 +23,9 @@
 #include "fft_core.cuh"
 #include <math.h>
 
+#include <algorithm>
+#include <cstdio>
+
 namespace {
 
 constexpr int kThreads = 256;
@@ -216,6 +219,275 @@ int mel_launch(MelParams p, cudaStream_t stream) {
   return EAT_OK;
 }
 
+// ---- backward: dspec [B, n_mels, T] -> dwave [B, N], the adjoint of mel_kernel (masks, affine, log, filterbank, power,
+// real FFT, window, overlap-add, reflect padding, pre-emphasis).  The frame spectra are recomputed, not stored.
+//
+// mel_bwd_kernel<M>: the forward's tiling (F frames of one clip per CTA, groups of M/8 threads per frame).  Per frame:
+// the forward FFT gives X[k], k = 0..M, and the mel energies; dmel = dspec / (5 (mel + 1e-5)) (0 where masked);
+// dpow[k] = sum_m fb[m, k] dmel[m], gathered per bin over the filters that cover it (s_first / s_last), so no bin is
+// written twice; dframe[i] = sum_k 2 dpow[k] Re(X[k] e^{+2 pi i k i / n_fft}) over the one-sided spectrum, which is the
+// unnormalised inverse real DFT of the Hermitian spectrum Z[k] = dpow[k] X[k] (k = 1..M-1), Z[0] = 2 dpow[0] X[0],
+// Z[M] = 2 dpow[M] X[M].  It runs as the same M-point complex FFT (fft_core.cuh) on conj(A + iB) with
+// A[k] = Z[k] + conj(Z[M-k]), B[k] = (Z[k] - conj(Z[M-k])) e^{+2 pi i k / n_fft}: the conjugated result holds the even
+// samples in its real and the odd samples in its imaginary parts.  The windowed frame gradients of a round are added
+// into the CTA's slice of the padded-signal gradient in group order (one CTA barrier per round), and the slice is
+// written to `work` [B][CTAs][seg_len].  mel_bwd_gather_kernel sums, for every waveform sample, the slices that overlap
+// each padded position that reads it (reflect padding folded back) in a fixed order and applies the pre-emphasis'
+// adjoint.  No floating-point atomics: the result is bitwise repeatable.
+struct MelBwdParams {
+  const float* dspec;    // [B, n_mels, T]
+  const float* wave;     // [B, N]
+  const float* window;
+  const float2* twiddle;
+  const int* fb_start;
+  const int* fb_len;
+  const float* fb_w;
+  const int *fs, *fe, *ts, *te;   // [B] SpecAugment bands of the forward, or all null
+  float* work;           // [B, ceil(T / F), seg_len]
+  int B, N, T, n_mels, win_length, hop, seg_len;
+  float preemph, log_offset, out_div;
+};
+
+template <int M>
+__global__ void __launch_bounds__(kThreads) mel_bwd_kernel(MelBwdParams p) {
+  using S = MelShape<M>;
+  constexpr int G = S::kGroupThreads, F = S::kFrames, NF = S::kNfft, NG = S::kGroups;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  float2* s_tw = reinterpret_cast<float2*>(smem_raw);                 // n_fft float2
+  float2* s_fft = s_tw + NF;                                          // NG * M float2
+  float2* s_X = s_fft + NG * M;                                       // NG * (M + 4) float2: X[k], then Z[k]
+  float* s_win = reinterpret_cast<float*>(s_X + NG * (M + 4));        // n_fft floats, zero-padded window
+  float* s_pow = s_win + NF;                                          // NG * (M + 4) floats: power, then dpow
+  int* s_first = reinterpret_cast<int*>(s_pow + NG * S::kPow);        // M + 4: first / last filter covering bin k
+  int* s_last = s_first + (M + 4);
+  float* s_g = reinterpret_cast<float*>(s_last + (M + 4));            // n_mels * (F + 1): dspec tile, then dmel
+  float* s_acc = s_g + p.n_mels * (F + 1);                            // seg_len: gradient of the padded signal slice
+
+  const int tid = threadIdx.x;
+  const int grp = tid >> S::kLog2Group;
+  const int j = tid & (G - 1);
+  const int b = blockIdx.y;
+  const int t_base = blockIdx.x * F;
+  const float* __restrict__ x = p.wave + (size_t)b * p.N;
+  const int L = p.N - 1;
+  const int lp = (NF - p.win_length) / 2;
+
+  for (int i = tid; i < NF; i += kThreads) {
+    s_tw[i] = p.twiddle[i];
+    int wi = i - lp;
+    s_win[i] = (wi >= 0 && wi < p.win_length) ? p.window[wi] : 0.f;
+  }
+  for (int k = tid; k <= M; k += kThreads) { s_first[k] = p.n_mels; s_last[k] = -1; }
+  for (int i = tid; i < p.seg_len; i += kThreads) s_acc[i] = 0.f;
+  for (int i = tid; i < p.n_mels * F; i += kThreads) {
+    const int m = i / F, fo = i % F, t = t_base + fo;
+    float g = 0.f;
+    if (t < p.T) {
+      const bool masked = p.fs != nullptr && ((m >= p.fs[b] && m < p.fe[b]) || (t >= p.ts[b] && t < p.te[b]));
+      g = masked ? 0.f : p.dspec[((size_t)b * p.n_mels + m) * p.T + t];
+    }
+    s_g[m * (F + 1) + fo] = g;
+  }
+  __syncthreads();
+  for (int m = tid; m < p.n_mels; m += kThreads) {
+    const int st = __ldg(p.fb_start + m), len = __ldg(p.fb_len + m);
+    for (int i = 0; i < len; ++i) { atomicMin(s_first + st + i, m); atomicMax(s_last + st + i, m); }
+  }
+  __syncthreads();
+
+  float2* zf = s_fft + grp * M;
+  float2* zx = s_X + grp * (M + 4);
+  float* pw = s_pow + grp * S::kPow;
+
+  for (int round = 0; round < F / NG; ++round) {
+    const int fl = round * NG + grp;
+    const int t = t_base + fl;
+    const bool live = t < p.T;                 // uniform within a group
+    float2 v[8];
+    // ---- recompute the frame's spectrum: the forward's passes
+    if (live) {
+      const int s0 = t * p.hop - M;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        const int n = j + G * r;
+        v[r] = make_float2(s_win[2 * n] * preemph_sample(x, s0 + 2 * n, L, p.preemph),
+                           s_win[2 * n + 1] * preemph_sample(x, s0 + 2 * n + 1, L, p.preemph));
+      }
+    }
+#pragma unroll
+    for (int pass = 0; pass < 2; ++pass) {
+      // pass 0: forward FFT of the windowed frame; pass 1: the inverse of the spectrum gradient (v = conj(A + iB))
+      if (live) {
+        stockham8_compute_m(v, j, 1, M, s_tw);
+#pragma unroll
+        for (int r = 0; r < 8; ++r) zf[stockham8_dst(j, 1, r)] = v[r];
+      }
+      group_sync<G>(grp);
+#pragma unroll
+      for (int Ns = 8; Ns < S::kRadix8End; Ns *= 8) {
+        if (live) {
+#pragma unroll
+          for (int r = 0; r < 8; ++r) v[r] = zf[j + G * r];
+          stockham8_compute_m(v, j, Ns, M, s_tw);
+        }
+        group_sync<G>(grp);
+        if (live) {
+#pragma unroll
+          for (int r = 0; r < 8; ++r) zf[stockham8_dst(j, Ns, r)] = v[r];
+        }
+        group_sync<G>(grp);
+      }
+      if constexpr (S::kTail != 1) {
+        if (live) {
+#pragma unroll
+          for (int r = 0; r < 8; ++r) v[r] = zf[j + G * r];
+          if constexpr (S::kTail == 2) stockham2_tail(v, j, M, s_tw);
+          else stockham4_tail(v, j, M, s_tw);
+#pragma unroll
+          for (int r = 0; r < 8; ++r) zf[j + G * r] = v[r];
+        }
+        group_sync<G>(grp);
+      }
+      if (pass == 1) break;
+      // ---- spectrum and power, bins 0..M
+      if (live) {
+#pragma unroll
+        for (int r = 0; r < 8; ++r) {
+          const int k = j + G * r;
+          const float2 X = rfft_split(zf[k], zf[(M - k) & (M - 1)], s_tw[M + k]);
+          zx[k] = X;
+          pw[k] = X.x * X.x + X.y * X.y;
+        }
+        if (j == 0) { const float2 z0 = zf[0]; const float nyq = z0.x - z0.y; zx[M] = make_float2(nyq, 0.f); pw[M] = nyq * nyq; }
+      }
+      group_sync<G>(grp);
+      // ---- mel energies as the forward computes them -> dmel, in place of the dspec tile
+      if (live) {
+        for (int m = j; m < p.n_mels; m += G) {
+          const int st = __ldg(p.fb_start + m), len = __ldg(p.fb_len + m);
+          float acc = 0.f;
+          for (int i = 0; i < len; ++i) acc = fmaf(__ldg(p.fb_w + (size_t)i * p.n_mels + m), pw[st + i], acc);
+          s_g[m * (F + 1) + fl] /= p.out_div * (acc + p.log_offset);
+        }
+      }
+      group_sync<G>(grp);
+      // ---- dpow per bin (transposed filterbank), Z[k] = dpow[k] X[k] (twice at k = 0 and M)
+      if (live) {
+        for (int k = j; k <= M; k += G) {
+          float d = 0.f;
+          for (int m = s_first[k]; m <= s_last[k]; ++m) {
+            const int i = k - __ldg(p.fb_start + m);
+            if (i >= 0 && i < __ldg(p.fb_len + m)) d = fmaf(__ldg(p.fb_w + (size_t)i * p.n_mels + m), s_g[m * (F + 1) + fl], d);
+          }
+          if (k == 0 || k == M) d *= 2.f;
+          zx[k] = make_float2(zx[k].x * d, zx[k].y * d);
+        }
+      }
+      group_sync<G>(grp);
+      if (live) {
+#pragma unroll
+        for (int r = 0; r < 8; ++r) {
+          const int k = j + G * r;
+          const float2 zk = zx[k], zm = zx[M - k];
+          const float2 a = make_float2(zk.x + zm.x, zk.y - zm.y);
+          const float2 w = make_float2(s_tw[M + k].x, -s_tw[M + k].y);       // e^{+2 pi i k / n_fft}
+          const float2 bb = cmul(make_float2(zk.x - zm.x, zk.y + zm.y), w);
+          v[r] = make_float2(a.x - bb.y, -(a.y + bb.x));                     // conj(A + iB)
+        }
+      }
+      group_sync<G>(grp);                       // zf is rewritten by the inverse's first pass
+    }
+    // ---- windowed frame gradient, in place: float2 n of zf becomes floats 2n, 2n+1
+    if (live) {
+      float* df = reinterpret_cast<float*>(zf);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        const int n = j + G * r;
+        const float2 c = zf[n];
+        df[2 * n] = s_win[2 * n] * c.x;
+        df[2 * n + 1] = -s_win[2 * n + 1] * c.y;
+      }
+    }
+    __syncthreads();
+    // ---- overlap-add of the round's frames into the slice, in group order
+    for (int i = tid; i < p.seg_len; i += kThreads) {
+      float a = s_acc[i];
+#pragma unroll
+      for (int g = 0; g < NG; ++g) {
+        const int f2 = round * NG + g, o = i - f2 * p.hop;
+        if (t_base + f2 < p.T && o >= 0 && o < NF) a += reinterpret_cast<const float*>(s_fft + g * M)[o];
+      }
+      s_acc[i] = a;
+    }
+    __syncthreads();
+  }
+  float* out = p.work + ((size_t)b * gridDim.x + blockIdx.x) * p.seg_len;
+  for (int i = tid; i < p.seg_len; i += kThreads) out[i] = s_acc[i];
+}
+
+// dwave[b, n] = gp[n-1] - preemph * gp[n] (pre-emphasis p[q] = x[q+1] - c x[q], q < L = N-1), where gp[q] sums the
+// padded-signal gradient over the positions s in [-M, (T-1) hop + M) that read p[q] (s = q, -q, 2(L-1) - q), each
+// the sum of the CTA slices covering it, in slice order
+__global__ void mel_bwd_gather_kernel(const float* __restrict__ work, float* __restrict__ dwave, int B, int N, int T,
+                                      int hop, int M, int frames, int seg_len, int ctas, float preemph) {
+  const long long n_all = (long long)B * N;
+  const int L = N - 1, span = frames * hop, s_end = (T - 1) * hop + M;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n_all; idx += (long long)gridDim.x * blockDim.x) {
+    const int b = (int)(idx / N), n = (int)(idx % N);
+    const float* wb = work + (size_t)b * ctas * seg_len;
+    auto at = [&](int s) {                      // gradient of padded position s
+      float a = 0.f;
+      if (s < -M || s >= s_end) return a;
+      const int u = s + M;
+      const int c_hi = min(ctas - 1, u / span), c_lo = u >= seg_len ? (u - seg_len) / span + 1 : 0;
+      for (int c = c_lo; c <= c_hi; ++c) a += __ldg(wb + (size_t)c * seg_len + (u - c * span));
+      return a;
+    };
+    auto gp = [&](int q) {
+      float a = at(q);
+      if (q > 0) a += at(-q);
+      if (q < L - 1) a += at(2 * (L - 1) - q);
+      return a;
+    };
+    float d = 0.f;
+    if (n >= 1) d = gp(n - 1);
+    if (n < L) d = fmaf(-preemph, gp(n), d);
+    dwave[idx] = d;
+  }
+}
+
+template <int M>
+size_t mel_bwd_smem(int n_mels, int seg_len) {
+  using S = MelShape<M>;
+  return S::kNfft * (sizeof(float2) + sizeof(float)) +
+         S::kGroups * (M * sizeof(float2) + (M + 4) * sizeof(float2) + S::kPow * sizeof(float)) +
+         2 * (M + 4) * sizeof(int) + ((size_t)n_mels * (S::kFrames + 1) + (size_t)seg_len) * sizeof(float);
+}
+
+template <int M>
+int mel_bwd_launch(MelBwdParams p, float* dwave, long long work_floats, cudaStream_t stream) {
+  using S = MelShape<M>;
+  const long long seg_len = (long long)(S::kFrames - 1) * p.hop + S::kNfft;
+  const size_t smem = mel_bwd_smem<M>(p.n_mels, (int)std::min(seg_len, (long long)INT32_MAX));
+  if (seg_len > INT32_MAX || smem > kSmemCap) {
+    eat_set_error("eat_mel_bwd: hop too large for the shared-memory signal slice"); return EAT_ERR_UNSUPPORTED;
+  }
+  const int ctas = ceil_div(p.T, S::kFrames);
+  if (work_floats < (long long)p.B * ctas * seg_len) { eat_set_error("eat_mel_bwd: work too small"); return EAT_ERR_ARG; }
+  if (p.B == 0) return EAT_OK;
+  p.seg_len = (int)seg_len;
+  static unsigned long long attr_mask = 0;
+  if (int rc = eat_opt_in_smem(mel_bwd_kernel<M>, kSmemCap, attr_mask)) return rc;
+  mel_bwd_kernel<M><<<dim3(ctas, p.B), kThreads, smem, stream>>>(p);
+  EAT_CHECK_LAUNCH();
+  const long long n_all = (long long)p.B * p.N;
+  const int grid = (int)std::min((long long)kNumSMs * 16, (n_all + 255) / 256);
+  mel_bwd_gather_kernel<<<grid, 256, 0, stream>>>(p.work, dwave, p.B, p.N, p.T, p.hop, M, S::kFrames, p.seg_len, ctas,
+                                                  p.preemph);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
 // training-time SpecAugment bands (torchaudio Frequency/TimeMasking, iid per example): positions inside
 // [fs,fe) x all t or all f x [ts,te) are overwritten with `fill`.
 __global__ void mel_mask_kernel(float* __restrict__ spec, int B, int F, int T, const int* __restrict__ fs,
@@ -305,5 +577,61 @@ extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window,
     case 1024: return mel_launch<512>(p, stream);
     case 2048: return mel_launch<1024>(p, stream);
     default: return mel_launch<2048>(p, stream);
+  }
+}
+
+namespace {
+int mel_geometry_check(const char* who, int B, int N, int win_length, int hop, int n_fft, int n_mels) {
+  char msg[160];
+  int rc = EAT_OK;
+  if (n_fft != 256 && n_fft != 512 && n_fft != 1024 && n_fft != 2048 && n_fft != 4096) {
+    snprintf(msg, sizeof msg, "%s: n_fft must be one of 256, 512, 1024, 2048, 4096", who); rc = EAT_ERR_UNSUPPORTED;
+  } else if (win_length > n_fft || win_length < 1 || hop < 1 || n_mels < 1 || n_mels > 512 || B < 0) {
+    snprintf(msg, sizeof msg, "%s: bad geometry", who); rc = EAT_ERR_ARG;
+  } else if (N - 1 <= n_fft / 2) {
+    snprintf(msg, sizeof msg, "%s: waveform too short for reflect padding", who); rc = EAT_ERR_ARG;
+  }
+  if (rc != EAT_OK) eat_set_error(msg);
+  return rc;
+}
+int mel_frames_per_cta(int n_fft) { return n_fft == 4096 ? MelShape<2048>::kFrames : MelShape<128>::kFrames; }
+}  // namespace
+
+extern "C" int eat_mel_bwd_workspace(int B, int N, int hop, int n_fft, long long* floats) {
+  if (int rc = mel_geometry_check("eat_mel_bwd_workspace", B, N, n_fft, hop, n_fft, 1)) return rc;
+  if (floats == nullptr) { eat_set_error("eat_mel_bwd_workspace: floats is null"); return EAT_ERR_ARG; }
+  const int F = mel_frames_per_cta(n_fft), T = 1 + (N - 1) / hop;
+  *floats = (long long)B * ((T + F - 1) / F) * ((long long)(F - 1) * hop + n_fft);
+  return EAT_OK;
+}
+
+extern "C" int eat_mel_bwd(const float* dspec, const float* wave, int B, int N, const float* window, int win_length, int hop,
+                           int n_fft, const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w,
+                           int max_len, int n_mels, float preemph, const int* f_start, const int* f_end,
+                           const int* t_start, const int* t_end, float* work, long long work_floats, float* dwave,
+                           cudaStream_t stream) {
+  if (int rc = mel_geometry_check("eat_mel_bwd", B, N, win_length, hop, n_fft, n_mels)) return rc;
+  const bool masks = f_start != nullptr || f_end != nullptr || t_start != nullptr || t_end != nullptr;
+  if (masks && (f_start == nullptr || f_end == nullptr || t_start == nullptr || t_end == nullptr)) {
+    eat_set_error("eat_mel_bwd: the four mask bounds are given together or not at all"); return EAT_ERR_ARG;
+  }
+  if (B > 0 && (dspec == nullptr || wave == nullptr || window == nullptr || twiddle == nullptr || fb_start == nullptr ||
+                fb_len == nullptr || fb_w == nullptr || work == nullptr || dwave == nullptr)) {
+    eat_set_error("eat_mel_bwd: dspec, wave, window, twiddle, the filterbank, work and dwave are required");
+    return EAT_ERR_ARG;
+  }
+  (void)max_len;
+  MelBwdParams p;
+  p.dspec = dspec; p.wave = wave; p.window = window; p.twiddle = reinterpret_cast<const float2*>(twiddle);
+  p.fb_start = fb_start; p.fb_len = fb_len; p.fb_w = fb_w;
+  p.fs = f_start; p.fe = f_end; p.ts = t_start; p.te = t_end; p.work = work;
+  p.B = B; p.N = N; p.T = 1 + (N - 1) / hop; p.n_mels = n_mels; p.win_length = win_length; p.hop = hop; p.seg_len = 0;
+  p.preemph = preemph; p.log_offset = 1e-5f; p.out_div = 5.f;
+  switch (n_fft) {
+    case 256: return mel_bwd_launch<128>(p, dwave, work_floats, stream);
+    case 512: return mel_bwd_launch<256>(p, dwave, work_floats, stream);
+    case 1024: return mel_bwd_launch<512>(p, dwave, work_floats, stream);
+    case 2048: return mel_bwd_launch<1024>(p, dwave, work_floats, stream);
+    default: return mel_bwd_launch<2048>(p, dwave, work_floats, stream);
   }
 }

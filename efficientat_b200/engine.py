@@ -34,6 +34,11 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _stat_ptrs(stats):
+    """(sum, sq) pointers of a statistics accumulator, or nulls when the forward runs on running statistics"""
+    return (0, 0) if stats is None else (stats[0].data_ptr(), stats[1].data_ptr())
+
+
 def _conv_out(n, k, s, d=1):
     return (n + 2 * ((k - 1) // 2) * d - d * (k - 1) - 1) // s + 1
 
@@ -121,6 +126,10 @@ class _Fork:
 
 class MNEngine:
     mha = None          # the MultiHeadAttentionPooling classifier, when the model has that head instead of 'mlp' (see _plan)
+    # The saving forward and its backward in eval mode (input gradients): every BatchNorm runs on its running statistics,
+    # whose backward is the batch-statistics formula with c1 = c2 = 0 (see _bn_bwd_coef)
+    _bn_frozen = False
+    _unwanted = frozenset()     # ids of gradient views no one asked for: the launches that only fill them are skipped
 
     def __init__(self, model):
         self.model = model
@@ -240,7 +249,10 @@ class MNEngine:
         return sc
 
     def _finalize(self, bn, stats, count, dev):
-        """batch statistics -> (scale/shift [2,C], saved mean/invstd [2,C]); updates running buffers."""
+        """batch statistics -> (scale/shift [2,C], saved mean/invstd [2,C]); updates running buffers.
+        On running statistics (_bn_frozen): the folded scale/shift and the running mean/invstd; no buffer changes."""
+        if self._bn_frozen:
+            return self._fold(bn, dev), torch.stack((bn.running_mean, torch.rsqrt(bn.running_var + bn.eps)))
         c = bn.num_features
         sc = torch.empty(2, c, device=dev, dtype=torch.float32)
         sv = torch.empty(2, c, device=dev, dtype=torch.float32)
@@ -282,16 +294,26 @@ class MNEngine:
             raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
         check_module_tensors(self.model, x.device, type(self.model).__name__)
         self.dropout_p = head_dropout(self.model)                    # read at call time (it may be changed after engine())
-        needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.model.parameters())
+        return self._dispatch(x, return_fmaps)
+
+    def _dispatch(self, x, return_fmaps):
+        """train(): batch-statistics forward, with a graph when a parameter or the input requires grad.  eval(): the folded
+        forward without a graph, unless the input requires grad: then the saving forward on running statistics."""
+        from .autograd import mn_eval_grad_forward, mn_train_forward
+        grad_on = torch.is_grad_enabled()
+        input_grad = grad_on and x.requires_grad
+        needs_grad = input_grad or (grad_on and any(p.requires_grad for p in self.model.parameters()))
         with torch.cuda.device(x.device):                            # launches go to x's device, whatever is current
             if self.model.training:
                 if return_fmaps:
                     raise NotImplementedError("return_fmaps is available in eval mode only")
-                from .autograd import mn_train_forward
                 logits, feat = mn_train_forward(self, x, needs_grad)
                 return self._squeeze(logits, feat) + (None,)
-            if needs_grad and x.requires_grad:
-                raise NotImplementedError("gradients w.r.t. the input spectrogram are not implemented")
+            if input_grad:
+                if return_fmaps:
+                    raise NotImplementedError("return_fmaps is not available when the input requires grad")
+                logits, feat = mn_eval_grad_forward(self, x)
+                return self._squeeze(logits, feat) + (None,)
             logits, feat, fmaps = self._forward_eval(x.detach(), return_fmaps)
             return self._squeeze(logits, feat) + (fmaps,)
 
@@ -388,11 +410,20 @@ class MNEngine:
 
     # ------------------------------------------------------------------ training forward
     def _new_stats(self, c, dev):
-        return self._zero_pool.take(2, c, dev)
+        return None if self._bn_frozen else self._zero_pool.take(2, c, dev)
 
-    def _forward_train(self, x, dropout_mask=None):
+    def _forward_train(self, x, dropout_mask=None, frozen=False):
         """Batch-statistics forward.  Returns (logits, feat, saved) where `saved` holds the raw conv outputs
-        and BatchNorm statistics needed by `_backward` (activations are recomputed from them)."""
+        and BatchNorm statistics needed by `_backward` (activations are recomputed from them).
+        frozen: the same forward with every BatchNorm on its running statistics (no buffer update) and no dropout --
+        eval mode's forward when the input's gradient is wanted."""
+        self._bn_frozen = frozen
+        try:
+            return self._forward_train_impl(x, dropout_mask)
+        finally:
+            self._bn_frozen = False
+
+    def _forward_train_impl(self, x, dropout_mask):
         L = lib()
         dev = x.device
         st = _stream()
@@ -400,7 +431,7 @@ class MNEngine:
         x = x.detach().float().contiguous()
         B, _, F, T = x.shape
         HS = ACT["hswish"]
-        S = {"x": x, "B": B, "F": F, "T": T, "blocks": []}
+        S = {"x": x, "B": B, "F": F, "T": T, "blocks": [], "frozen": self._bn_frozen}
         self._zero_pool = _ZeroPool()
 
         conv, bn = self.stem[0], self.stem[1]
@@ -409,8 +440,7 @@ class MNEngine:
         c0 = conv.out_channels
         z0 = torch.empty(B, Fi, Ti, c0, device=dev, dtype=td)
         stt = self._new_stats(c0, dev)
-        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), z0.data_ptr(), dc, B, F, T, c0, s0, 0, 0, 0,
-                   stt[0].data_ptr(), stt[1].data_ptr(), st)
+        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), z0.data_ptr(), dc, B, F, T, c0, s0, 0, 0, 0, *_stat_ptrs(stt), st)
         sc0, sv0 = self._finalize(bn, stt, B * Fi * Ti, dev)
         a = torch.empty_like(z0)
         L.bn_apply(z0.data_ptr(), sc0[0].data_ptr(), sc0[1].data_ptr(), HS, 0, a.data_ptr(), dc, B * Fi * Ti, c0, st)
@@ -449,10 +479,10 @@ class MNEngine:
               blk.act if dw_sc is not None else 0)
         if blk.dil > 1:
             L.dw_conv_fwd_dil(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
-                              blk.dil, *xf, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+                              blk.dil, *xf, 0, 0, 0, 0, *_stat_ptrs(stt), st)
         else:
             L.dw_conv_fwd(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, *xf,
-                          0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+                          0, 0, 0, 0, *_stat_ptrs(stt), st)
         sc2, sv2 = self._finalize(blk.dw[1], stt, Mo, dev)
         R.update(z2=z2, sc2=sc2, sv2=sv2, wt=wt, Fo=Fo, To=To)
         gate = None
@@ -498,7 +528,7 @@ class MNEngine:
         n1 = self.fc1.out_features
         h_pre = torch.empty(B, n1, device=dev, dtype=torch.float32)
         self._gemm(feat, self.fc1.weight, h_pre, B, n1, cl, bias=self.fc1.bias, a_code=0, c_code=0)
-        p = self.dropout_p
+        p = 0.0 if self._bn_frozen else self.dropout_p
         if dropout_mask is None and p > 0:
             dropout_mask = torch.empty(B, n1, device=dev, dtype=torch.float32).bernoulli_(1.0 - p).div_(1.0 - p)
         ident = self._ident(n1, dev)
@@ -565,8 +595,14 @@ class MNEngine:
     def param_list(self):
         return [p for p in self.model.parameters()]
 
+    def _wanted(self, grad):
+        """the gradient view, or None when its parameter's gradient was not asked for"""
+        return None if grad is None or id(grad) in self._unwanted else grad
+
     def _wgrad(self, g, a, dW, db, M, N, K, in_sc=None, in_act=0, gate=None, rows_per_sample=1, g_code=None,
                a_code=None):
+        if self._wanted(dW) is None and self._wanted(db) is None:
+            return
         g_code = self.dcode if g_code is None else g_code
         a_code = self.dcode if a_code is None else a_code
         args = (g.data_ptr(), g_code, a.data_ptr(), a_code, dW.data_ptr(), _ptr(db), M, N, K,
@@ -583,6 +619,15 @@ class MNEngine:
         """BatchNorm-backward reduce (unless `sums` holds it already) + finalize -> the apply pass's (c1, c2) [2, C]"""
         L = lib()
         st = _stream()
+        count = float(B * P)
+        if self._bn_frozen:
+            # running statistics do not depend on the batch: c1 = c2 = 0, and the apply is dz = scale * dy * act'.  The
+            # reduce (against the running mean and invstd) only serves gamma's and beta's gradients; an infinite count
+            # makes eat_bn_bwd_finalize's c1 = s1 / count and c2 = s2 / count zero
+            dgamma, dbeta = self._wanted(dgamma), self._wanted(dbeta)
+            if dgamma is None and dbeta is None:
+                return torch.zeros(2, C, device=dev, dtype=torch.float32)
+            count = float("inf")
         if sums is None:
             s = self._zero_pool.take(2, C, dev)
             L.bn_bwd_reduce(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
@@ -590,21 +635,22 @@ class MNEngine:
         else:
             s = sums
         coef = torch.empty(2, C, device=dev, dtype=torch.float32)
-        L.bn_bwd_finalize(s[0].data_ptr(), s[1].data_ptr(), float(B * P), _ptr(dgamma), _ptr(dbeta),
+        L.bn_bwd_finalize(s[0].data_ptr(), s[1].data_ptr(), count, _ptr(dgamma), _ptr(dbeta),
                           coef[0].data_ptr(), coef[1].data_ptr(), C, st)
         return coef
 
     def _bn_bwd(self, gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code=None, sums=None):
         """two-pass BatchNorm(+activation) backward -> dz (same dtype/shape as z).  `sums`: the (s1, s2) accumulators when
         the reduce pass already happened elsewhere (SE blocks: eat_se_bn_bwd_reduce + eat_se_bn_bwd_combine)."""
-        L = lib()
-        st = _stream()
         code = self.dcode if code is None else code
         coef = self._bn_bwd_coef(gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code, sums)
+        return self._bn_bwd_apply(gA, gate, dpool, z, sc, sv, act, coef, B, P, C, code)
+
+    def _bn_bwd_apply(self, gA, gate, dpool, z, sc, sv, act, coef, B, P, C, code):
         dz = torch.empty_like(z)
-        L.bn_bwd_apply(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
-                       sv[0].data_ptr(), sv[1].data_ptr(), act, coef[0].data_ptr(), coef[1].data_ptr(), dz.data_ptr(),
-                       code, B, P, C, st)
+        lib().bn_bwd_apply(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
+                           sv[0].data_ptr(), sv[1].data_ptr(), act, coef[0].data_ptr(), coef[1].data_ptr(), dz.data_ptr(),
+                           code, B, P, C, _stream())
         return dz
 
     def _block_bwd(self, blk, R, dy, G, B):
@@ -693,7 +739,9 @@ class MNEngine:
         dz2 = self._bn_bwd(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
                            G[blk.dw[1].weight], G[blk.dw[1].bias], dev, sums=sums2)
         xf = (_ptr(sc1[0]) if has_exp else 0, _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0)
-        if blk.dil > 1:
+        if self._wanted(G[blk.dw[0].weight]) is None:
+            pass                                        # the depthwise weight's gradient was not asked for
+        elif blk.dil > 1:
             fork.run(lambda: L.dw_conv_wgrad_dil(dz2.data_ptr(), dw_in.data_ptr(), *xf, G[blk.dw[0].weight].data_ptr(), dc,
                                                  B, Fi, Ti, blk.cexp, blk.k, blk.stride, blk.dil, _stream()), dz2)
         else:
@@ -761,10 +809,21 @@ class MNEngine:
                 self._pw_bwd_ok[key] = False
         return self._pw_bwd_ok[key]
 
-    def _backward(self, S, dlogits, on_ready=None):
+    def _backward(self, S, dlogits, on_ready=None, input_grad=False, wanted=None):
         """-> dict {parameter: fp32 gradient view into one flat arena} (arena returned under key None).
         on_ready(flat, i): called after each stage with the index i of the first parameter (model.parameters() order)
-        whose gradient is final -- everything from i to the end is -- so a data-parallel trainer can start reducing."""
+        whose gradient is final -- everything from i to the end is -- so a data-parallel trainer can start reducing.
+        input_grad: the input spectrogram's gradient [B, 1, F, T] fp32 is returned under key "x".  wanted: the parameters
+        whose gradients are needed (None: all); launches that only produce the others' gradients are skipped, so their
+        views hold no gradient.  A forward on running statistics (S["frozen"]) gets the backward on them."""
+        self._bn_frozen = S["frozen"]
+        try:
+            return self._backward_impl(S, dlogits, on_ready, input_grad, wanted)
+        finally:
+            self._bn_frozen = False
+            self._unwanted = frozenset()
+
+    def _backward_impl(self, S, dlogits, on_ready, input_grad, wanted):
         L = lib()
         st = _stream()
         dev = dlogits.device
@@ -778,6 +837,9 @@ class MNEngine:
         for p in params:
             G[p] = flat[off:off + p.numel()].view_as(p)
             off += p.numel()
+        if wanted is not None:
+            wanted = {id(p) for p in wanted}
+            self._unwanted = frozenset(id(G[p]) for p in params if id(p) not in wanted)
         dlogits = dlogits.float().contiguous()
         fork = self._fork = _Fork(dev, self.fork_wgrad)
         pidx = {id(p): i for i, p in enumerate(params)}
@@ -796,7 +858,7 @@ class MNEngine:
             done(self.model.classifier)
             dz = self._bn_bwd(gA, None, None, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, conv.out_channels, G[bn.weight],
                               G[bn.bias], dev)
-            return self._backward_trunk(S, G, flat, fork, done, dz)
+            return self._backward_trunk(S, G, flat, fork, done, dz, input_grad)
         H = S["head"]
         n1, ncls, cl = self.fc1.out_features, self.fc2.out_features, self.fc1.in_features
         fork.run(lambda: self._wgrad(dlogits, H["h_pre"], G[self.fc2.weight], G[self.fc2.bias], B, ncls, n1, in_sc=H["ident"],
@@ -813,9 +875,9 @@ class MNEngine:
         # ---- last 1x1 conv (+BN+Hardswish, global average pool)
         dpool = dfeat.mul_(1.0 / P)      # gradient of the spatial mean, broadcast inside the BN-backward kernels
         dz = self._bn_bwd(None, None, dpool, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, cl, G[bn.weight], G[bn.bias], dev)
-        return self._backward_trunk(S, G, flat, fork, done, dz)
+        return self._backward_trunk(S, G, flat, fork, done, dz, input_grad)
 
-    def _backward_trunk(self, S, G, flat, fork, done, dz):
+    def _backward_trunk(self, S, G, flat, fork, done, dz, input_grad=False):
         """from the gradient dz at the last 1x1 conv's output down to the stem"""
         L = lib()
         st = _stream()
@@ -840,13 +902,27 @@ class MNEngine:
         St = S["stem"]
         conv, bn = self.stem[0], self.stem[1]
         c0 = conv.out_channels
-        if self.stem_bwd_fused and dc == 0 and c0 <= 64 and c0 % 4 == 0 and conv.stride[0] in (1, 2):
-            # dz0 is computed on load in its only consumer and never stored
-            coef = self._bn_bwd_coef(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0,
-                                     G[bn.weight], G[bn.bias], dev, 0, None)
-            L.stem_wgrad(dy.data_ptr(), 0, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
-                         conv.stride[0], St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
-                         St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(), st)
+        P0 = St["Fo"] * St["To"]
+        fused = self.stem_bwd_fused and dc == 0 and c0 <= 64 and c0 % 4 == 0 and conv.stride[0] in (1, 2)
+        if fused or input_grad:
+            coef = self._bn_bwd_coef(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, P0, c0, G[bn.weight], G[bn.bias],
+                                     dev, dc, None)
+            wgrad = self._wanted(G[conv.weight]) is not None
+            if wgrad and fused:
+                # dz0 is computed on load in its only consumer and never stored
+                L.stem_wgrad(dy.data_ptr(), 0, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
+                             conv.stride[0], St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
+                             St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(), st)
+            elif wgrad:
+                dz0 = self._bn_bwd_apply(dy, None, None, St["z"], St["sc"], St["sv"], HS, coef, B, P0, c0, dc)
+                L.stem_wgrad(dz0.data_ptr(), dc, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
+                             conv.stride[0], 0, 0, 0, 0, 0, 0, 0, 0, st)
+            if input_grad:
+                dx = torch.empty(B, 1, S["F"], S["T"], device=dev, dtype=torch.float32)
+                L.stem_dgrad(dy.data_ptr(), dc, St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
+                             St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(),
+                             conv.weight.data_ptr(), dx.data_ptr(), B, S["F"], S["T"], c0, conv.stride[0], st)
+                G["x"] = dx
         else:
             dz0 = self._bn_bwd(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0, G[bn.weight],
                                G[bn.bias], dev)

@@ -10,7 +10,7 @@ reductions, the coefficient / attention / coordinate nets, and the ContextGen po
 import torch
 
 from ._lib import check_module_tensors, lib
-from .engine import ACT, MNEngine, _Layer, _conv_out, _ptr, _stream
+from .engine import ACT, MNEngine, _Layer, _conv_out, _ptr, _stat_ptrs, _stream
 
 
 class DyMNEngine(MNEngine):
@@ -53,16 +53,7 @@ class DyMNEngine(MNEngine):
             raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
         check_module_tensors(self.model, x.device, type(self.model).__name__)
         self.dropout_p = float(self.model.classifier[4].p)
-        with torch.cuda.device(x.device):
-            if self.model.training:
-                if return_fmaps:
-                    raise NotImplementedError("return_fmaps is available in eval mode only")
-                needs_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.model.parameters())
-                from .autograd import mn_train_forward
-                logits, feat = mn_train_forward(self, x, needs_grad)
-                return logits, feat, None
-            logits, feat, fmaps = self._forward_eval(x.detach(), return_fmaps)
-            return logits, feat, fmaps
+        return self._dispatch(x, return_fmaps)
 
     # ------------------------------------------------------------------ DynamicConv 1x1 dispatch
     def _mixed_weights(self, W, att, B, n):
@@ -286,10 +277,10 @@ class DyMNEngine(MNEngine):
               blk.act if dw_sc is not None else 0)
         if npc == 2:
             L.dw_conv_fwd_dy(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
-                             s, *xs, 0, 0, 0, 0, 0, 0, 0, stt[0].data_ptr(), stt[1].data_ptr(), st)
+                             s, *xs, 0, 0, 0, 0, 0, 0, 0, *_stat_ptrs(stt), st)
         else:
             L.dw_conv_fwd_dy_m(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp,
-                               blk.k, s, *xs, 0, 0, 0, 0, 0, 0, 0, npc, stt[0].data_ptr(), stt[1].data_ptr(), st)
+                               blk.k, s, *xs, 0, 0, 0, 0, 0, 0, 0, npc, *_stat_ptrs(stt), st)
         sc2, sv2 = self._finalize(m.depth_norm, stt, Mo, dev)
         p = torch.empty_like(z2)
         act_args = (z2.data_ptr(), p.data_ptr(), dc, sc2[0].data_ptr(), sc2[1].data_ptr(), theta.data_ptr(),

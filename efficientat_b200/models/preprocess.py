@@ -2,7 +2,9 @@
 
 Same constructor, buffers, RNG side effects and output as reference models/preprocess.py:6-67;
 the seven library calls of its forward (:41-65) are one launch of eat_mel_fwd (csrc/mel.cu).
+A waveform that requires grad gets its gradient from eat_mel_bwd, with the filterbank and masks of the forward call.
 """
+import ctypes
 import math
 
 import torch
@@ -82,14 +84,16 @@ class AugmentMelSTFT(nn.Module):
             self._fb_cache[key] = hit
         return hit
 
-    def _device_filterbank(self, fmin, fmax, device):
+    def _device_filterbank(self, fmin, fmax, device, private=False):
+        """private: a filterbank of this call's own, kept for its backward (the shared buffer is rebuilt every call)"""
         cap = self.n_fft // 2 + 1
-        buf = getattr(self, "_fb_dev", None)
+        buf = None if private else getattr(self, "_fb_dev", None)
         if buf is None or buf[0].device != device:
             buf = (torch.empty(self.n_mels, dtype=torch.int32, device=device),
                    torch.empty(self.n_mels, dtype=torch.int32, device=device),
                    torch.empty(cap, self.n_mels, dtype=torch.float32, device=device))
-            self._fb_dev = buf
+            if not private:
+                self._fb_dev = buf
         lib().mel_filterbank(self.n_mels, self.n_fft, float(self.sr), float(fmin), float(fmax), buf[0].data_ptr(),
                              buf[1].data_ptr(), buf[2].data_ptr(), cap, torch.cuda.current_stream().cuda_stream)
         return buf[0], buf[1], buf[2], cap
@@ -100,11 +104,13 @@ class AugmentMelSTFT(nn.Module):
         if x.dim() != 2:
             raise ValueError(f"expected waveform of shape [B, N], got {tuple(x.shape)}")
         check_module_tensors(self, x.device, "AugmentMelSTFT")
-        x = x.float().contiguous()
         with torch.cuda.device(x.device):
-            return self._forward(x)
+            if torch.is_grad_enabled() and x.requires_grad:
+                return _MelFn.apply(self, x)
+            return self._forward(x.float().contiguous())
 
-    def _forward(self, x):
+    def _forward(self, x, saved=None):
+        """saved: a dict that receives the filterbank and masks of this call, for eat_mel_bwd"""
         # the reference draws both randints on every call, eval included (preprocess.py:45-46)
         fmin = self.fmin + torch.randint(self.fmin_aug_range, (1,)).item()
         fmax = self.fmax + self.fmax_aug_range // 2 - torch.randint(self.fmax_aug_range, (1,)).item()
@@ -112,7 +118,7 @@ class AugmentMelSTFT(nn.Module):
             fmin, fmax = self.fmin, self.fmax
         if self.training and (self.fmin_aug_range > 1 or self.fmax_aug_range > 1):
             # jittered filterbank: build it on the device, no host work or copy in the step
-            start, length, taps, max_len = self._device_filterbank(fmin, fmax, x.device)
+            start, length, taps, max_len = self._device_filterbank(fmin, fmax, x.device, private=saved is not None)
         else:
             start, length, taps, max_len = self._filterbank(fmin, fmax, x.device)
         b, n = x.shape
@@ -132,4 +138,45 @@ class AugmentMelSTFT(nn.Module):
                 # masks are applied in the log domain before the affine, i.e. value (0 + 4.5) / 5 = 0.9
                 lib().mel_mask(out.data_ptr(), b, self.n_mels, t, fs.data_ptr(), fe.data_ptr(), ts.data_ptr(),
                                te.data_ptr(), 0.9, torch.cuda.current_stream().cuda_stream)
+                if saved is not None:
+                    saved["masks"] = (fs, fe, ts, te)
+        if saved is not None:
+            saved.update(fb=(start, length, taps, max_len))
         return out
+
+    def _backward(self, x, dspec, saved):
+        b, n = x.shape
+        start, length, taps, max_len = saved["fb"]
+        masks = saved.get("masks")
+        L = lib()
+        st = torch.cuda.current_stream().cuda_stream
+        need = ctypes.c_longlong()
+        L.mel_bwd_workspace(b, n, self.hopsize, self.n_fft, ctypes.addressof(need))
+        work = torch.empty(need.value, device=x.device, dtype=torch.float32)
+        dx = torch.empty_like(x)
+        L.mel_bwd(dspec.data_ptr(), x.data_ptr(), b, n, self.window.data_ptr(), self.win_length, self.hopsize, self.n_fft,
+                  self._twiddle.data_ptr(), start.data_ptr(), length.data_ptr(), taps.data_ptr(), max_len, self.n_mels,
+                  self._preemph, *([m.data_ptr() for m in masks] if masks is not None else [0, 0, 0, 0]),
+                  work.data_ptr(), work.numel(), dx.data_ptr(), st)
+        return dx
+
+
+class _MelFn(torch.autograd.Function):
+    """waveform -> log-mel with the waveform's gradient from eat_mel_bwd (fp32; the frame spectra are recomputed)"""
+
+    @staticmethod
+    def forward(ctx, module, x):
+        x = x.detach().float().contiguous()
+        saved = {}
+        out = module._forward(x, saved)
+        ctx.module, ctx.x, ctx.saved = module, x, saved
+        return out
+
+    @staticmethod
+    def backward(ctx, dspec):
+        if torch.is_grad_enabled():
+            raise NotImplementedError("double backward (create_graph=True) through AugmentMelSTFT is not implemented")
+        with torch.cuda.device(ctx.x.device):
+            dx = ctx.module._backward(ctx.x, dspec.float().contiguous(), ctx.saved)
+        ctx.x = ctx.saved = None
+        return None, dx

@@ -74,6 +74,21 @@ int eat_mel_fwd(const float* wave, int B, int N, const float* window, int win_le
                 const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len,
                 int n_mels, float preemph, float* out, cudaStream_t stream);
 
+/* Adjoint of eat_mel_fwd (with eat_mel_mask's bands): dspec [B, n_mels, T] fp32 -> dwave [B, N] fp32 (overwritten), the
+ * gradient through the affine, the masks (zero where the forward masked), log(mel + 1e-5), the banded filterbank, the
+ * power spectrum, the real FFT, the window, the overlap-add of the frames, the reflect padding and the pre-emphasis.
+ * wave, window, twiddle and the filterbank are the forward call's; the frame spectra are recomputed.  f_start, f_end,
+ * t_start, t_end [B] int32: the forward's SpecAugment bands, all four or none.  work: eat_mel_bwd_workspace floats of
+ * scratch.  Bitwise repeatable (no floating-point atomics).  Geometry checks as eat_mel_fwd; a hop whose slice does not
+ * fit in shared memory -> EAT_ERR_UNSUPPORTED, a short work -> EAT_ERR_ARG.  All checks precede any launch; B = 0 is a
+ * no-op. */
+int eat_mel_bwd(const float* dspec, const float* wave, int B, int N, const float* window, int win_length, int hop,
+                int n_fft, const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len,
+                int n_mels, float preemph, const int* f_start, const int* f_end, const int* t_start, const int* t_end,
+                float* work, long long work_floats, float* dwave, cudaStream_t stream);
+/* Host-only: the floats of scratch eat_mel_bwd needs for B clips of N samples. */
+int eat_mel_bwd_workspace(int B, int N, int hop, int n_fft, long long* floats);
+
 /* Kaldi mel filterbank in banded form, built on the device (training-mode fmin/fmax jitter,
  * models/preprocess.py:45-55 + torchaudio.compliance.kaldi.get_mel_banks).  fb_w holds cap x n_mels floats. */
 int eat_mel_filterbank(int n_mels, int n_fft, float sample_rate, double fmin, double fmax, int* fb_start,
@@ -382,6 +397,16 @@ int eat_pw_proj_bwd_plan(long long M, int cexp, int cout, int* plan);
 int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, int F, int T, int C, int stride,
                    const float* z, const float* scale, const float* shift, const float* mean, const float* invstd, int act,
                    const float* c1, const float* c2, cudaStream_t stream);
+/* Stem data gradient, the adjoint of eat_stem_fwd's 3x3 conv: dy [B,Fo,To,C] (dtype) is the gradient at the stem
+ * BatchNorm + activation's output and z [B,Fo,To,C] (dtype) the raw conv output; the conv output's gradient
+ * eat_bn_bwd_apply(dy, NULL, NULL, z, scale, shift, mean, invstd, act, c1, c2) is computed on load and never stored.
+ * c1 = c2 = 0 with the running statistics' scale, shift, mean and invstd is the backward of a BatchNorm in eval mode.
+ * w [C,1,3,3] fp32 -> dx [B,F,T] fp32 (overwritten).  Bitwise repeatable (no atomics).  C as eat_stem_fwd (a multiple
+ * of 4 (fp32) or 8 (bf16), at most 256 vectors), F, T >= 1, act none/relu/hardswish and every pointer given, else
+ * EAT_ERR_ARG; stride other than 1 or 2 -> EAT_ERR_UNSUPPORTED.  All checks precede any launch; B = 0 is a no-op. */
+int eat_stem_dgrad(const void* dy, int dtype, const void* z, const float* scale, const float* shift, const float* mean,
+                   const float* invstd, int act, const float* c1, const float* c2, const float* w, float* dx, int B, int F,
+                   int T, int C, int stride, cudaStream_t stream);
 /* dpre = dh * mask * act'(pre), fp32 vectors (classifier Hardswish + Dropout backward). */
 int eat_act_bwd(const float* dh, const float* pre, const float* mask, int act, float* dpre, long long n,
                 cudaStream_t stream);
