@@ -221,29 +221,43 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
     const int ctid = threadIdx.x - kFirstCons * 32;           // 0..255
     unsigned char* stg = s_stg + (size_t)cw * p.stg_bufs * STG_BYTES;
     const int bnp = p.bnp;
-    float* my_stat = s_stat + cw * 2 * bnp;
     const bool do_stats = EPI == 0 && p.stat_sum != nullptr;
     const uint64_t desc0 = gmma_desc(0);                      // descriptor of address 0: add (address >> 4)
     const uint64_t wres0 = desc0 + (smem_u32(s_w) >> 4);
     const uint32_t w_tile16 = w_tile >> 4;
-    float csum[NC], csq[NC];
+    // Batch statistics: a lane sums d = x - K and d^2 over its column in fp32, K the first value it summed, and the
+    // combine adds the shift back in fp64.  A lane sums its column over every tile of the CTA (~7,800 values at mn10
+    // block 2 with 256 clips of 10 s); unshifted fp32 sums of x^2 lose the variance to cancellation in E[x^2] - E[x]^2
+    // when the column's mean is many times its std.
+    float csum[NC], csq[NC], ck[NC];
+    int cn[NC];
 #pragma unroll
-    for (int c = 0; c < NC; ++c) { csum[c] = 0.f; csq[c] = 0.f; }
+    for (int c = 0; c < NC; ++c) { csum[c] = 0.f; csq[c] = 0.f; ck[c] = 0.f; cn[c] = 0; }
     int cur_nt = -1, cb = 0, s = 0;
     uint32_t ph = 0;
     auto flush_stats = [&](int nt_old) {
-      // lane partials -> shared, combine the eight warps, one fp64 atomic per channel (lanes past a tail chunk hold 0)
+      // lane partials -> fp64 sums of x and x^2 in shared, combine the eight warps in fp64, one fp64 atomic per channel
+      // (lanes past a tail chunk hold 0); the table holds one of the two sums at a time
+      double* s_d = reinterpret_cast<double*>(s_stat);      // [8 warps][bnp]
 #pragma unroll
-      for (int c = 0; c < NC; ++c) { my_stat[c * 32 + lane] = csum[c]; my_stat[bnp + c * 32 + lane] = csq[c]; csum[c] = 0.f; csq[c] = 0.f; }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int e = ctid; e < BN; e += kConsThreads) {
-        const int n = nt_old * BN + e;
-        float a = 0.f, b = 0.f;
+      for (int q = 0; q < 2; ++q) {
 #pragma unroll
-        for (int w = 0; w < 8; ++w) { a += s_stat[w * 2 * bnp + e]; b += s_stat[w * 2 * bnp + bnp + e]; }
-        if (n < p.N) { atomicAdd(p.stat_sum + n, (double)a); atomicAdd(p.stat_sq + n, (double)b); }
+        for (int c = 0; c < NC; ++c) {
+          const double k = ck[c], n = cn[c], d1 = csum[c];
+          s_d[cw * bnp + c * 32 + lane] = q == 0 ? d1 + n * k : (double)csq[c] + k * (2.0 * d1 + n * k);
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        for (int e = ctid; e < BN; e += kConsThreads) {
+          const int n = nt_old * BN + e;
+          double a = 0.0;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) a += s_d[w * bnp + e];
+          if (n < p.N) atomicAdd((q == 0 ? p.stat_sum : p.stat_sq) + n, a);
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+      for (int c = 0; c < NC; ++c) { csum[c] = 0.f; csq[c] = 0.f; ck[c] = 0.f; cn[c] = 0; }
     };
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int bs, jt;
@@ -370,12 +384,18 @@ pw_tma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ 
             // lane = column: sum the staged column over the rows of this slab that lie inside M
             float s1 = 0.f, s2 = 0.f;
             const int cj = lane >> 2, ci = lane & 3;
-            if (lane < cw) {
-              for (int r = 0; r < rows_left; ++r) {
+            if (lane < cw && rows_left > 0) {
+              auto at = [&](int r) {
                 const uint32_t o = tail ? (uint32_t)(r * cw + lane) * 4 : (uint32_t)(r * 128 + ((cj ^ (r & 7)) << 4) + ci * 4);
-                const float x = *reinterpret_cast<const float*>(buf + o);
-                s1 += x; s2 = fmaf(x, x, s2);
+                return *reinterpret_cast<const float*>(buf + o);
+              };
+              if (cn[c] == 0) ck[c] = at(0);
+              const float k = ck[c];
+              for (int r = 0; r < rows_left; ++r) {
+                const float d = at(r) - k;
+                s1 += d; s2 = fmaf(d, d, s2);
               }
+              cn[c] += rows_left;
             }
             csum[c] += s1; csq[c] += s2;
           }
@@ -491,16 +511,19 @@ constexpr size_t kSmemLimit = 227 * 1024;
 
 struct Maps { CUtensorMap A, W, C, Ct, R; };
 
+// persistent grid, a multiple of n_tiles (the kernel's tile walk); the tile count m_tiles * n_tiles is one as well
+int plan_grid(const TmaParams& p, int sms) {
+  return min(p.m_tiles * p.n_tiles, max(p.n_tiles, sms / p.n_tiles * p.n_tiles));
+}
+
 template <int EPI, int XACT, int BN>
-int launch_kernel(const Maps& m, const TmaParams& p, size_t smem, int tiles, cudaStream_t st) {
+int launch_kernel(const Maps& m, const TmaParams& p, size_t smem, cudaStream_t st) {
   static unsigned long long attr_mask = 0;
   if (int rc = eat_opt_in_smem(pw_tma_kernel<EPI, XACT, BN>, kSmemLimit, attr_mask)) return rc;
   int dev = 0, sms = kNumSMs;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // persistent grid, a multiple of n_tiles (the kernel's tile walk); tiles is one as well
-  const int grid = min(tiles, max(p.n_tiles, sms / p.n_tiles * p.n_tiles));
-  pw_tma_kernel<EPI, XACT, BN><<<grid, kThreads, smem, st>>>(m.A, m.W, m.C, m.Ct, m.R, p);
+  pw_tma_kernel<EPI, XACT, BN><<<plan_grid(p, sms), kThreads, smem, st>>>(m.A, m.W, m.C, m.Ct, m.R, p);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }
@@ -521,28 +544,33 @@ constexpr int fit_width(std::integer_sequence<int, W...>, int bn) {
 }
 
 template <int EPI, int XACT, int... W>
-int launch_width(std::integer_sequence<int, W...>, const Maps& m, const TmaParams& p, size_t smem, int tiles, cudaStream_t st) {
+int launch_width(std::integer_sequence<int, W...>, const Maps& m, const TmaParams& p, size_t smem, cudaStream_t st) {
   int rc = EAT_ERR_UNSUPPORTED;
-  const bool found = ((p.BN == W && (rc = launch_kernel<EPI, XACT, W>(m, p, smem, tiles, st), true)) || ...);
+  const bool found = ((p.BN == W && (rc = launch_kernel<EPI, XACT, W>(m, p, smem, st), true)) || ...);
   if (!found) eat_set_error("pw_tma: no kernel for this tile width");
   return rc;
 }
 
 struct WeightWs { int trans; void* ws; size_t bytes; const float* att; int dyn_k; };   // att != nullptr: DynamicConv kernel mix
 
-template <int EPI, int XACT>
-int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams p, cudaStream_t st, WeightWs ws) {
-  // ---- tiling.  Every N tile lands and fixes up the A tile again (TMA write 16 KB + fix-up 32 KB per k-block), so N is
-  // cut into as few tiles as the consumer registers allow (a 64 x 128 fp32 accumulator per warpgroup = 64 registers per
-  // thread), of equal width rounded up to 8 columns: tensor-core work is padded by at most 7 columns per tile.  A width
-  // without a compiled kernel runs on the next wider one (the TMA unit zero-fills the weight rows past N).
+// ---- tiling.  Every N tile lands and fixes up the A tile again (TMA write 16 KB + fix-up 32 KB per k-block), so N is
+// cut into as few tiles as the consumer registers allow (a 64 x 128 fp32 accumulator per warpgroup = 64 registers per
+// thread), of equal width rounded up to 8 columns: tensor-core work is padded by at most 7 columns per tile.  A width
+// without a compiled kernel runs on the next wider one (the TMA unit zero-fills the weight rows past N).
+template <int EPI>
+void plan_tiles(TmaParams& p) {
   p.n_tiles = ceil_div(p.N, BN_MAX);
   p.BN = fit_width(Widths<EPI>{}, (ceil_div(p.N, p.n_tiles) + 7) & ~7);
   p.n_tiles = ceil_div(p.N, p.BN);
-  p.bnp = BN_MAX;
   if (p.n_samples < 1) { p.n_samples = 1; p.tile_rps = p.M; }
   p.tps = ceil_div(p.tile_rps, BM);
   p.m_tiles = p.n_samples * p.tps;
+}
+
+template <int EPI, int XACT>
+int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams p, cudaStream_t st, WeightWs ws) {
+  plan_tiles<EPI>(p);
+  p.bnp = BN_MAX;
   p.k_blocks = ceil_div(p.K, KB);
   p.r_blocks = R != nullptr ? ceil_div(min(p.BN, p.N), 32) : 0;
   p.kpad = XACT >= 0 ? p.k_blocks * KB : 0;
@@ -605,7 +633,7 @@ int launch_tma(const void* A, const float* W, void* C, const void* R, TmaParams 
     m.Ct = mC;                                               // unused: every chunk is a full one
   }
   if (int rc = make_map3(&mR, R != nullptr ? R : C, ns, rps, p.N, BM, 4)) return rc;
-  return launch_width<EPI, XACT>(Widths<EPI>{}, m, p, smem, p.m_tiles * p.n_tiles, st);
+  return launch_width<EPI, XACT>(Widths<EPI>{}, m, p, smem, st);
 }
 
 template <int EPI>
@@ -674,4 +702,20 @@ extern "C" int eat_pw_tma_dyn_fwd(const float* A, const float* W, const float* a
   if (act == EAT_ACT_RELU) return launch_tma_x<2>(A, W, C, residual, p, st, ws);
   if (act == EAT_ACT_HSWISH) return launch_tma_x<3>(A, W, C, residual, p, st, ws);
   return launch_tma_x<1>(A, W, C, residual, p, st, ws);
+}
+
+extern "C" int eat_pw_tma_plan(long long M, int N, int K, int rows_per_sample, int raw, int sms, int* plan) {
+  if (plan == nullptr) { eat_set_error("pw_tma_plan: plan is NULL"); return EAT_ERR_ARG; }
+  if (M < 1 || N < 1 || K < 1 || sms < 1) { eat_set_error("pw_tma_plan: M, N, K and sms must be positive"); return EAT_ERR_ARG; }
+  if (M >= (1ll << 31) - BM) { eat_set_error("pw_tma_plan: M too large"); return EAT_ERR_ARG; }
+  if (rows_per_sample > 0 && M % rows_per_sample != 0) { eat_set_error("pw_tma_plan: M must be B * rows_per_sample"); return EAT_ERR_ARG; }
+  TmaParams p{};
+  p.M = (int)M; p.N = N; p.K = K;
+  if (rows_per_sample > 0) { p.n_samples = (int)(M / rows_per_sample); p.tile_rps = rows_per_sample; }
+  if (raw) plan_tiles<0>(p);
+  else plan_tiles<1>(p);
+  const int grid = plan_grid(p, sms);
+  plan[0] = p.BN; plan[1] = p.n_tiles; plan[2] = p.m_tiles; plan[3] = grid;
+  plan[4] = ceil_div(p.m_tiles * p.n_tiles, grid);
+  return EAT_OK;
 }

@@ -139,7 +139,10 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
   float* s_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);      // 8 warps x 32 x STG_LD floats
   float* s_scale = s_stage + 8 * 32 * STG_LD;                                  // [BN_MAX]
   float* s_shift = s_scale + BN_MAX;                                           // [BN_MAX]
-  float* s_stat = s_shift + BN_MAX;                                            // [8 warps][2][BN_MAX]
+  // [8 warps][2][BN_MAX] statistics partials, fp64: a warp adds one 16-row partial per tile to them, over every tile of
+  // the CTA (~480 at mn10 block 2 with 256 clips of 10 s); in fp32 the sum of squares would lose the variance to
+  // cancellation in E[x^2] - E[x]^2 when the column's mean is many times its std
+  double* s_stat = reinterpret_cast<double*>(s_shift + BN_MAX);
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_stat + 8 * 2 * BN_MAX);       // full[S], empty[S]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -151,7 +154,7 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, kGroupThreads / 32); mbar_init(bar_empty + 8 * s, 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  for (int i = threadIdx.x; i < 8 * 2 * BN_MAX; i += kThreads) s_stat[i] = 0.f;
+  for (int i = threadIdx.x; i < 8 * 2 * BN_MAX; i += kThreads) s_stat[i] = 0.0;
   __syncthreads();
 
   const int total_tiles = p.m_tiles * p.n_tiles;
@@ -320,8 +323,8 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
     const int g = ew >> 2;                                        // 64-row half of the tile
     const int wq = ew & 3;                                        // rows 16 wq .. 16 wq + 15 of the half
     float* stg = s_stage + ew * 32 * STG_LD;
-    float* my_sum = s_stat + ew * 2 * BN_MAX;
-    float* my_sq = my_sum + BN_MAX;
+    double* my_sum = s_stat + ew * 2 * BN_MAX;
+    double* my_sq = my_sum + BN_MAX;
     T* __restrict__ C = reinterpret_cast<T*>(p.C);
     const T* __restrict__ R = reinterpret_cast<const T*>(p.residual);
     const int etid = threadIdx.x - kFirstCons * 32;               // 0..255
@@ -345,12 +348,12 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
         for (int i = etid; i < BN; i += kEpiThreads) {
           if (do_stats && cur_nt >= 0) {
             const int n = cur_nt * BN + i;
-            float a = 0.f, b = 0.f;
+            double a = 0.0, b = 0.0;
 #pragma unroll
             for (int w = 0; w < 8; ++w) { a += s_stat[w * 2 * BN_MAX + i]; b += s_stat[w * 2 * BN_MAX + BN_MAX + i]; }
-            if (n < N) { atomicAdd(p.stat_sum + n, (double)a); atomicAdd(p.stat_sq + n, (double)b); }
+            if (n < N) { atomicAdd(p.stat_sum + n, a); atomicAdd(p.stat_sq + n, b); }
 #pragma unroll
-            for (int w = 0; w < 8; ++w) { s_stat[w * 2 * BN_MAX + i] = 0.f; s_stat[w * 2 * BN_MAX + BN_MAX + i] = 0.f; }
+            for (int w = 0; w < 8; ++w) { s_stat[w * 2 * BN_MAX + i] = 0.0; s_stat[w * 2 * BN_MAX + BN_MAX + i] = 0.0; }
           }
           const int n = n0 + i;
           s_scale[i] = (p.scale != nullptr && n < N) ? p.scale[n] : 1.f;
@@ -465,7 +468,7 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
           }
           if (lane < 8 && cl < BN) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) { my_sum[cl + j] += cs[j]; my_sq[cl + j] += cq[j]; }
+            for (int j = 0; j < 4; ++j) { my_sum[cl + j] += (double)cs[j]; my_sq[cl + j] += (double)cq[j]; }
           }
         }
         __syncwarp();
@@ -476,10 +479,10 @@ __global__ void __launch_bounds__(kThreads, 1) pw_tc_kernel(TcParams p) {
     if (do_stats && cur_nt >= 0) {
       for (int i = etid; i < BN; i += kEpiThreads) {
         const int n = cur_nt * BN + i;
-        float a = 0.f, b = 0.f;
+        double a = 0.0, b = 0.0;
 #pragma unroll
         for (int w = 0; w < 8; ++w) { a += s_stat[w * 2 * BN_MAX + i]; b += s_stat[w * 2 * BN_MAX + BN_MAX + i]; }
-        if (n < N) { atomicAdd(p.stat_sum + n, (double)a); atomicAdd(p.stat_sq + n, (double)b); }
+        if (n < N) { atomicAdd(p.stat_sum + n, a); atomicAdd(p.stat_sq + n, b); }
       }
     }
   }
@@ -501,7 +504,7 @@ int launch_tc_x(const TcParams& p0, cudaStream_t st) {
   }
   p.k_blocks = ceil_div(p.K, BK);
   constexpr size_t smem = (size_t)STAGES * NP * (A_TILE_BYTES + BN_MAX * 128) + 8 * 32 * STG_LD * sizeof(float) +
-                          2 * BN_MAX * sizeof(float) + 16 * BN_MAX * sizeof(float) +
+                          2 * BN_MAX * sizeof(float) + 16 * BN_MAX * sizeof(double) +
                           2 * STAGES * sizeof(uint64_t) + 16;
   static_assert(smem <= 227 * 1024, "shared memory budget");
   static unsigned long long attr_mask = 0;

@@ -34,6 +34,10 @@ constexpr int GB = 2;                   // G boxes per stage: 64 output channels
 constexpr int XB = 2;                   // X boxes per stage at most: 64 input channels -> 128 accumulator columns
 constexpr int kThreads = 416;
 constexpr int kFirstCons = 4, kTmaWarp = 12;
+// The register accumulators are flushed to dW (and restarted) every kFlushRows reduction rows: the tensor core's fp32
+// accumulation rounds toward zero, so a long split with same-signed terms drifts by ~1.5 x 2^-24 of the sum per 16-row
+// step; over 31k rows (mn10 block 2 at B = 256) that was 1.5e-4 of sum |terms|, within 30x of a dropped 128-row block.
+constexpr int kFlushRows = 4096;
 
 struct WgParams {
   float* dW;
@@ -136,7 +140,7 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant
       if (++s == S) { s = 0; ph ^= 1u; }
     }
   } else {
-    // ================================================================= consumers: MMA, then once per CTA the atomics
+    // ================================================================= consumers: MMA, the atomics every kFlushRows rows
     const int cw = warp - kFirstCons;
     const int g = cw >> 2, wq = cw & 3;                        // G box of this warpgroup, warp inside it
     const int ctid = threadIdx.x - kFirstCons * 32;
@@ -145,6 +149,33 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant
     for (int b = 0; b < XB; ++b)
 #pragma unroll
       for (int i = 0; i < 32; ++i) acc[b][i] = 0.f;
+    // accumulator rows of this thread: r = 16 wq + lane / 4 (+ 8) inside the group's 64 rows [hi(n) 0..31 | lo(n) 0..31]
+    auto flush = [&]() {
+      if (g < gb) {
+        const bool hi_row = wq < 2;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = (wq & 1) * 16 + (lane >> 2) + 8 * h;          // channel inside the 32-channel box
+          const int n = n0 + g * 32 + r;
+          if (n >= p.N) continue;
+#pragma unroll
+          for (int b = 0; b < XB; ++b) {
+            if (b >= xb) continue;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {                             // hi(k) columns 8 j + 2 (lane % 4) of box b
+              const int k = k0 + b * KB + 8 * j + 2 * (lane & 3);
+              float2 v = make_float2(acc[b][4 * j + 2 * h], acc[b][4 * j + 2 * h + 1]);
+              if (hi_row) { v.x += acc[b][4 * (j + 4) + 2 * h]; v.y += acc[b][4 * (j + 4) + 2 * h + 1]; }   // + hi.lo
+              if (k < p.K) atomicAdd(reinterpret_cast<float2*>(dWout + (size_t)n * p.K + k), v);
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int b = 0; b < XB; ++b)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[b][i] = 0.f;
+    };
     int s = 0;
     uint32_t ph = 0;
     for (int blk = 0; blk < n_blocks; ++blk) {
@@ -172,50 +203,32 @@ wgrad_tma_kernel(const __grid_constant__ CUtensorMap mapG, const __grid_constant
       asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");   // every warp of the group is past its wait
       if (ctid == g * 128) mbar_arrive(bar_empty + 8 * s);
       if (++s == S) { s = 0; ph ^= 1u; }
+      if ((blk + 1) % (kFlushRows / MB) == 0 && blk + 1 < n_blocks) flush();
     }
-    // accumulator rows of this thread: r = 16 wq + lane / 4 (+ 8) inside the group's 64 rows [hi(n) 0..31 | lo(n) 0..31]
-    if (n_blocks > 0 && g < gb) {
-      const bool hi_row = wq < 2;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = (wq & 1) * 16 + (lane >> 2) + 8 * h;          // channel inside the 32-channel box
-        const int n = n0 + g * 32 + r;
-        if (n >= p.N) continue;
-#pragma unroll
-        for (int b = 0; b < XB; ++b) {
-          if (b >= xb) continue;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {                             // hi(k) columns 8 j + 2 (lane % 4) of box b
-            const int k = k0 + b * KB + 8 * j + 2 * (lane & 3);
-            float2 v = make_float2(acc[b][4 * j + 2 * h], acc[b][4 * j + 2 * h + 1]);
-            if (hi_row) { v.x += acc[b][4 * (j + 4) + 2 * h]; v.y += acc[b][4 * (j + 4) + 2 * h + 1]; }   // + hi.lo
-            if (k < p.K) atomicAdd(reinterpret_cast<float2*>(dWout + (size_t)n * p.K + k), v);
-          }
-        }
-      }
-    }
+    if (n_blocks > 0) flush();
   }
   __syncthreads();
 }
 
-template <int XACT, int MB>
-int launch_wg_mb(const float* G, const float* X, WgParams p, cudaStream_t st) {
-  constexpr int BOX = MB * 128;
+// The launch plan (fills the tiling / split / stage fields of p) -> MB and the number of reduction splits.  sms: the
+// GPU's SM count.  128-row blocks when a stage holds at most three boxes (N <= 64 and K <= 32, or N <= 32 and K <= 64)
+// and the reduction is long: the first layers of the network, M in the millions.
+int plan_wg(WgParams& p, int sms, int& mb, int& splits) {
   p.n_tiles = ceil_div(p.N, 64);
   p.k_tiles = ceil_div(p.K, XB * KB);
   const int kt = p.K < XB * KB ? p.K : XB * KB;
   p.xb = ceil_div(kt, KB);
-  int dev = 0, sms = kNumSMs;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  p.gbs = p.N <= KB ? 1 : GB;
+  const int boxes = p.gbs + p.xb;
+  mb = (boxes <= 3 && p.sample_rows == 0 && p.M >= (1 << 20)) ? 128 : 64;
+  if (const char* e = getenv("EAT_WG_MB")) { const int v = atoi(e); if (v == 64 || (v == 128 && boxes <= 3)) mb = v; }
   const int tiles = p.n_tiles * p.k_tiles;
   const int slots = sms;
-  int splits;
   if (p.sample_rows > 0) {
     const int B = p.M / p.sample_rows;
     int sps = max(1, (2 * slots) / max(1, tiles * B));
     long long rows = ceil_div_ll(p.sample_rows, sps);
-    rows = ceil_div_ll(rows, MB) * MB;
+    rows = ceil_div_ll(rows, mb) * mb;
     sps = (int)ceil_div_ll(p.sample_rows, rows);
     p.rows_per_split = (int)rows;
     p.splits_per_sample = sps;
@@ -223,41 +236,48 @@ int launch_wg_mb(const float* G, const float* X, WgParams p, cudaStream_t st) {
   } else {
     splits = max(1, (2 * slots) / tiles);
     long long rows = ceil_div_ll(p.M, splits);
-    rows = ceil_div_ll(rows, MB) * MB;
-    if (rows < 4 * MB) rows = 4 * MB;
+    rows = ceil_div_ll(rows, mb) * mb;
+    if (rows < 4 * mb) rows = 4 * mb;
     splits = (int)ceil_div_ll(p.M, rows);
     p.rows_per_split = (int)rows;
     p.splits_per_sample = 0;
   }
-  p.gbs = p.N <= KB ? 1 : GB;
-  p.stage_bytes = (uint32_t)((p.gbs + p.xb) * BOX);
+  p.stage_bytes = (uint32_t)(boxes * mb * 128);
   const size_t budget = 227 * 1024;
   const size_t misc = 2 * 64 * 4 + 3 * 8 * 8 + 16 + 1024;
   p.stages = (int)((budget - misc) / p.stage_bytes);
   if (p.stages > 8) p.stages = 8;
   if (p.stages < 2) { eat_set_error("wgrad_tma: shared-memory budget exceeded"); return EAT_ERR_UNSUPPORTED; }
+  return EAT_OK;
+}
+
+template <int XACT, int MB>
+int launch_wg_mb(const float* G, const float* X, const WgParams& p, int splits, cudaStream_t st) {
+  const size_t budget = 227 * 1024;
   size_t off = (size_t)p.stages * p.stage_bytes;
-  p.off_f = (uint32_t)off; off += 2 * 64 * 4;
-  p.off_bar = (uint32_t)off; off += 3 * (size_t)p.stages * 8 + 16;
+  const uint32_t off_f = (uint32_t)off; off += 2 * 64 * 4;
+  const uint32_t off_bar = (uint32_t)off; off += 3 * (size_t)p.stages * 8 + 16;
   const size_t smem = off;
+  WgParams q = p;
+  q.off_f = off_f; q.off_bar = off_bar;
   CUtensorMap mG, mX;
   if (int rc = make_map(&mG, G, p.M, p.N, MB)) return rc;
   if (int rc = make_map(&mX, X, p.M, p.K, MB)) return rc;
   static unsigned long long attr_mask = 0;
   if (int rc = eat_opt_in_smem(wgrad_tma_kernel<XACT, MB>, budget, attr_mask)) return rc;
-  wgrad_tma_kernel<XACT, MB><<<tiles * splits, kThreads, smem, st>>>(mG, mX, p);
+  wgrad_tma_kernel<XACT, MB><<<p.n_tiles * p.k_tiles * splits, kThreads, smem, st>>>(mG, mX, q);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }
 
 template <int XACT>
-int launch_wg(const float* G, const float* X, const WgParams& p, cudaStream_t st) {
-  // 128-row blocks when a stage holds at most three boxes (N <= 64 and K <= 32, or N <= 32 and K <= 64) and the
-  // reduction is long: the first layers of the network, M in the millions
-  const int boxes = (p.N <= KB ? 1 : GB) + ceil_div(p.K < XB * KB ? p.K : XB * KB, KB);
-  int mb = (boxes <= 3 && p.sample_rows == 0 && p.M >= (1 << 20)) ? 128 : 64;
-  if (const char* e = getenv("EAT_WG_MB")) { const int v = atoi(e); if (v == 64 || (v == 128 && boxes <= 3)) mb = v; }
-  return mb == 128 ? launch_wg_mb<XACT, 128>(G, X, p, st) : launch_wg_mb<XACT, 64>(G, X, p, st);
+int launch_wg(const float* G, const float* X, WgParams p, cudaStream_t st) {
+  int dev = 0, sms = kNumSMs;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int mb = 64, splits = 1;
+  if (int rc = plan_wg(p, sms, mb, splits)) return rc;
+  return mb == 128 ? launch_wg_mb<XACT, 128>(G, X, p, splits, st) : launch_wg_mb<XACT, 64>(G, X, p, splits, st);
 }
 
 int launch_wg_x(const float* G, const float* X, const WgParams& p, cudaStream_t st) {
@@ -288,4 +308,21 @@ extern "C" int eat_pw_tma_wgrad(const float* G, const float* X, float* dW, long 
     p.sample_rows = rows_per_sample;
   }
   return launch_wg_x(G, X, p, st);
+}
+
+extern "C" int eat_pw_wgrad_plan(long long M, int N, int K, int rows_per_sample, int per_sample, int sms, int* plan) {
+  if (plan == nullptr) { eat_set_error("pw_wgrad_plan: plan is NULL"); return EAT_ERR_ARG; }
+  if (M < 1 || N < 1 || K < 1 || sms < 1) { eat_set_error("pw_wgrad_plan: M, N, K and sms must be positive"); return EAT_ERR_ARG; }
+  if (M >= (1ll << 31) - 128) { eat_set_error("pw_wgrad_plan: M too large"); return EAT_ERR_ARG; }
+  WgParams p{};
+  p.M = (int)M; p.N = N; p.K = K;
+  if (per_sample) {
+    if (rows_per_sample < 1 || M % rows_per_sample != 0) { eat_set_error("pw_wgrad_plan: per-sample mode needs M = B * rows_per_sample"); return EAT_ERR_ARG; }
+    p.sample_rows = rows_per_sample;
+  }
+  int mb = 64, splits = 1;
+  if (int rc = plan_wg(p, sms, mb, splits)) return rc;
+  plan[0] = mb; plan[1] = p.n_tiles * p.k_tiles; plan[2] = splits; plan[3] = p.rows_per_split;
+  plan[4] = p.splits_per_sample; plan[5] = p.stages;
+  return EAT_OK;
 }

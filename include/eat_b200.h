@@ -176,6 +176,11 @@ int eat_pw_tma_dyn_fwd(const float* A, const float* W, const float* att, int dyn
                        int N, int K, int rows_per_sample, const float* scale, const float* shift, int act,
                        const float* residual, double* stat_sum, double* stat_sq, void* w_ws, long long w_ws_bytes,
                        cudaStream_t stream);
+/* Host-only (no GPU work): the tile walk eat_pw_tma_fwd (rows_per_sample = 0) / eat_pw_tma_dyn_fwd (rows_per_sample > 0:
+ * M tiles never straddle samples) launch on a GPU of sms SMs; raw != 0: the raw-output variant (training forward with
+ * batch statistics, data gradients), else an epilogue variant.  plan[5] = {N tile width, N tiles, M tiles, CTAs, M tiles
+ * of the CTA that takes the most}. */
+int eat_pw_tma_plan(long long M, int N, int K, int rows_per_sample, int raw, int sms, int* plan);
 /* out[cols, rows] = in[rows, cols]^T (fp32); used to feed W^T to the data-gradient GEMM. */
 int eat_transpose_f32(const float* in, float* out, int rows, int cols, cudaStream_t stream);
 
@@ -279,6 +284,10 @@ int eat_pw_tc_wgrad(const void* G, int g_dtype, const void* A, int a_dtype, floa
 int eat_pw_tma_wgrad(const float* G, const float* X, float* dW, long long M, int N, int K, const float* in_scale,
                      const float* in_shift, int in_act, const float* gate, int rows_per_sample, int per_sample,
                      cudaStream_t stream);
+/* Host-only: the launch plan of eat_pw_tma_wgrad for the same M, N, K, rows_per_sample, per_sample on a GPU of sms SMs.
+ * plan[6] = {reduction rows per pipeline stage (64 or 128), (64 x 64) dW tiles, reduction splits (CTAs per dW tile),
+ * rows per split, splits per sample (per-sample mode; 0 otherwise), pipeline stages}. */
+int eat_pw_wgrad_plan(long long M, int N, int K, int rows_per_sample, int per_sample, int sms, int* plan);
 
 /* BatchNorm backward, pass 1: s1[c] += sum dy, s2[c] += sum dy*xhat with dy = g * act'(z*scale+shift),
  * g = gA * gate[b,c] + dpool[b,c] (gA / gate / dpool each optional).  z, gA: [B, P, C]. */

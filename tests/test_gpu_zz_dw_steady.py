@@ -30,7 +30,7 @@ import torch
 import torch.nn.functional as Fn
 
 from efficientat_b200._lib import lib
-from tests.util import report
+from tests.util import bn_variance_check, report
 
 NONE, RELU, HS = 0, 1, 2
 F32, BF16 = 0, 1
@@ -243,27 +243,6 @@ def test_forward_training(case, dtype, in_act):
            f"stat_sq {u_q:.1f} x 2^-24 sum|terms|")
 
 
-def _variance_check(out, stats, ref, n, C, what):
-    """var + eps from eat_bn_finalize of the kernel's sums vs torch.var_mean (fp32) of the same output, both through an
-    fp32 invstd, against fp64"""
-    L = lib()
-    gamma, beta = torch.ones(C, device="cuda"), torch.zeros(C, device="cuda")
-    bn = torch.full((4, C), float("nan"), device="cuda")
-    L.bn_finalize(stats[0].contiguous().data_ptr(), stats[1].contiguous().data_ptr(), float(n), gamma.data_ptr(),
-                  beta.data_ptr(), EPS, 0.01, 0, 0, 0, bn[0].data_ptr(), bn[1].data_ptr(), bn[2].data_ptr(),
-                  bn[3].data_ptr(), C, _st())
-    mean64 = ref[0] / n
-    ve64 = ref[1] / n - mean64 * mean64 + EPS
-    var_t, _ = torch.var_mean(out.reshape(-1, C), dim=0, unbiased=False)
-    ve_t = 1.0 / torch.rsqrt(var_t + EPS).double() ** 2
-    ve_k = 1.0 / bn[3].double() ** 2
-    e_k = ((ve_k - ve64).abs() / ve64).max().item()
-    e_t = ((ve_t - ve64).abs() / ve64).max().item()
-    ratio = (mean64.abs() / (ve64 - EPS).clamp_min(1e-30).sqrt()).max().item()
-    report(f"[kernel] dw {what}: var + eps rel err kernel {e_k:.2e}, torch fp32 {e_t:.2e} (mean/std up to {ratio:.0f})")
-    assert e_k <= 2 * e_t, f"{what}: variance {e_k:.3e} relative vs torch fp32 {e_t:.3e}"
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", [FWD[1], FWD[5], FWD_STATS_BENCH], ids=_ids([FWD[1], FWD[5], FWD_STATS_BENCH]))
 def test_forward_statistics_keep_the_variance(case):
@@ -276,7 +255,7 @@ def test_forward_statistics_keep_the_variance(case):
     del x
     Fo, To = _out_hw(F, T, k, s)
     report(f"[kernel] dw fwd train dc {case}: output {e:.2e}, stat_sum {u_s:.1f} / stat_sq {u_q:.1f} x 2^-24 sum|terms|")
-    _variance_check(out, stats, ref, B * Fo * To, C, f"fwd train dc {case}")
+    bn_variance_check(out, stats, ref, B * Fo * To, C, EPS, f"dw fwd train dc {case}")
     peak = torch.cuda.max_memory_allocated() / 2 ** 30
     report(f"[kernel] dw fwd train dc {case}: peak device memory {peak:.2f} GiB")
     assert peak < 8, f"peak device memory {peak:.2f} GiB"

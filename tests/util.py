@@ -75,3 +75,26 @@ def topk_match(got, want, k=10, tie_tol=0.0):
             if gi[r] != wi[r] and abs(want[b, gi[r]] - want[b, wi[r]]) > tie_tol:
                 return False
     return True
+
+
+def bn_variance_check(out, stats, ref, n, C, eps, what, factor=2):
+    """var + eps from eat_bn_finalize of the kernel's sums vs torch.var_mean (fp32) of the same output, both through an
+    fp32 invstd, against fp64"""
+    from efficientat_b200._lib import lib
+    L = lib()
+    gamma, beta = torch.ones(C, device="cuda"), torch.zeros(C, device="cuda")
+    bn = torch.full((4, C), float("nan"), device="cuda")
+    L.bn_finalize(stats[0].contiguous().data_ptr(), stats[1].contiguous().data_ptr(), float(n), gamma.data_ptr(),
+                  beta.data_ptr(), eps, 0.01, 0, 0, 0, bn[0].data_ptr(), bn[1].data_ptr(), bn[2].data_ptr(),
+                  bn[3].data_ptr(), C, torch.cuda.current_stream().cuda_stream)
+    mean64 = ref[0] / n
+    ve64 = ref[1] / n - mean64 * mean64 + eps
+    var_t, _ = torch.var_mean(out.reshape(-1, C), dim=0, unbiased=False)
+    ve_t = 1.0 / torch.rsqrt(var_t + eps).double() ** 2
+    ve_k = 1.0 / bn[3].double() ** 2
+    e_k = ((ve_k - ve64).abs() / ve64).max().item()
+    e_t = ((ve_t - ve64).abs() / ve64).max().item()
+    ratio = (mean64.abs() / (ve64 - eps).clamp_min(1e-30).sqrt()).max().item()
+    report(f"[kernel] {what}: var + eps rel err kernel {e_k:.2e}, torch fp32 {e_t:.2e}, ratio {e_k / e_t:.2f} (bound {factor}; "
+           f"mean/std up to {ratio:.0f})")
+    assert e_k <= factor * e_t, f"{what}: variance {e_k:.3e} relative vs torch fp32 {e_t:.3e}"
