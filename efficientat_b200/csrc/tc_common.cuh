@@ -78,9 +78,9 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
       : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
 
-// m64nNk16 for any N = 8, 16, ..., 128, both operands K-major: d[N / 2] is the fragment above with j = 0 .. N / 8 - 1.
-// EAT_WG_S<N> / EAT_WG_O<N> spell out the N / 2 accumulator placeholders and operands; the descriptors and the scale-d
-// flag follow them as operands N / 2 .. N / 2 + 2.
+// m64nNk16 for any N = 8, 16, ..., 128: d[N / 2] is the fragment above with j = 0 .. N / 8 - 1; TA / TB as above (both
+// K-major by default).  EAT_WG_S<N> / EAT_WG_O<N> spell out the N / 2 accumulator placeholders and operands; the
+// descriptors, the scale-d flag and the two layout immediates follow them as operands N / 2 .. N / 2 + 4.
 #define EAT_WG_S8 "%0, %1, %2, %3"
 #define EAT_WG_S16 EAT_WG_S8 ", %4, %5, %6, %7"
 #define EAT_WG_S24 EAT_WG_S16 ", %8, %9, %10, %11"
@@ -113,18 +113,20 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
 #define EAT_WG_O112 EAT_WG_O104, "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
 #define EAT_WG_O120 EAT_WG_O112, "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59])
 #define EAT_WG_O128 EAT_WG_O120, "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-#define EAT_WG_CASE(W, DA, DB, ONE)                                                                                     \
+#define EAT_WG_CASE(W, DA, DB, ONE, TAI, TBI)                                                                           \
   if constexpr (N == W)                                                                                                 \
     asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #ONE ", 0;\n"                                                     \
-                 "wgmma.mma_async.sync.aligned.m64n" #W "k16.f32.bf16.bf16 {" EAT_WG_S##W "}, %" #DA ", %" #DB ", p, 1, 1, 0, 0;\n}\n" \
-                 : EAT_WG_O##W : "l"(da), "l"(db), "r"(1));
-template <int N>
+                 "wgmma.mma_async.sync.aligned.m64n" #W "k16.f32.bf16.bf16 {" EAT_WG_S##W "}, %" #DA ", %" #DB ", p, 1, 1, %" #TAI ", %" #TBI ";\n}\n" \
+                 : EAT_WG_O##W : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
+template <int N, int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma_kk(float (&d)[N / 2], uint64_t da, uint64_t db) {
   static_assert(N % 8 == 0 && N >= 8 && N <= 128, "m64nNk16: N is a multiple of 8 up to 128 here");
-  EAT_WG_CASE(8, 4, 5, 6) EAT_WG_CASE(16, 8, 9, 10) EAT_WG_CASE(24, 12, 13, 14) EAT_WG_CASE(32, 16, 17, 18)
-  EAT_WG_CASE(40, 20, 21, 22) EAT_WG_CASE(48, 24, 25, 26) EAT_WG_CASE(56, 28, 29, 30) EAT_WG_CASE(64, 32, 33, 34)
-  EAT_WG_CASE(72, 36, 37, 38) EAT_WG_CASE(80, 40, 41, 42) EAT_WG_CASE(88, 44, 45, 46) EAT_WG_CASE(96, 48, 49, 50)
-  EAT_WG_CASE(104, 52, 53, 54) EAT_WG_CASE(112, 56, 57, 58) EAT_WG_CASE(120, 60, 61, 62) EAT_WG_CASE(128, 64, 65, 66)
+  EAT_WG_CASE(8, 4, 5, 6, 7, 8) EAT_WG_CASE(16, 8, 9, 10, 11, 12) EAT_WG_CASE(24, 12, 13, 14, 15, 16)
+  EAT_WG_CASE(32, 16, 17, 18, 19, 20) EAT_WG_CASE(40, 20, 21, 22, 23, 24) EAT_WG_CASE(48, 24, 25, 26, 27, 28)
+  EAT_WG_CASE(56, 28, 29, 30, 31, 32) EAT_WG_CASE(64, 32, 33, 34, 35, 36) EAT_WG_CASE(72, 36, 37, 38, 39, 40)
+  EAT_WG_CASE(80, 40, 41, 42, 43, 44) EAT_WG_CASE(88, 44, 45, 46, 47, 48) EAT_WG_CASE(96, 48, 49, 50, 51, 52)
+  EAT_WG_CASE(104, 52, 53, 54, 55, 56) EAT_WG_CASE(112, 56, 57, 58, 59, 60) EAT_WG_CASE(120, 60, 61, 62, 63, 64)
+  EAT_WG_CASE(128, 64, 65, 66, 67, 68)
 }
 #undef EAT_WG_CASE
 

@@ -79,6 +79,71 @@ __device__ __forceinline__ void zero_upper(unsigned char* row, int cp, int x) {
   *reinterpret_cast<uint4*>(row + (((6 + cp) ^ x) << 4)) = z;
 }
 
+// The reading half of fix_a, for fix_pair: this thread's 8 fp32 values (va, vb) of each of its rows of a landed tile, with
+// the optional BatchNorm affine + activation (XACT >= 0) and SE gate applied and rows >= rows_valid forced to zero.
+// fix_a keeps its own copy so that the kernels built on it compile to the same instructions as before.
+template <int LG, int XACT, int TR>
+__device__ __forceinline__ void fix_load(const unsigned char* tile, int ft, int rows_valid, const float* s_isc,
+                                         const float* s_ish, int k, const float* gate, int off0, int b0, int rps, int K,
+                                         float4 (&va)[FixMap<LG, TR>::ROWS], float4 (&vb)[FixMap<LG, TR>::ROWS]) {
+  using M = FixMap<LG, TR>;
+  const int cp = ft & ((1 << LG) - 1), r0 = ft >> LG;
+  const uint32_t row_off = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128);
+  const int x = r0 & 7;
+  const uint32_t in0 = row_off + (((2 * cp) ^ x) << 4), in1 = row_off + (((2 * cp + 1) ^ x) << 4);
+#pragma unroll
+  for (int i = 0; i < M::ROWS; ++i) {
+    va[i] = *reinterpret_cast<const float4*>(tile + in0 + i * M::STRIDE);
+    vb[i] = *reinterpret_cast<const float4*>(tile + in1 + i * M::STRIDE);
+  }
+  if (XACT >= 0) {
+    const float4 sa = *reinterpret_cast<const float4*>(s_isc + k), sb = *reinterpret_cast<const float4*>(s_isc + k + 4);
+    const float4 ha = *reinterpret_cast<const float4*>(s_ish + k), hb = *reinterpret_cast<const float4*>(s_ish + k + 4);
+#pragma unroll
+    for (int i = 0; i < M::ROWS; ++i) {
+      va[i].x = act_in<XACT>(fmaf(va[i].x, sa.x, ha.x)); va[i].y = act_in<XACT>(fmaf(va[i].y, sa.y, ha.y));
+      va[i].z = act_in<XACT>(fmaf(va[i].z, sa.z, ha.z)); va[i].w = act_in<XACT>(fmaf(va[i].w, sa.w, ha.w));
+      vb[i].x = act_in<XACT>(fmaf(vb[i].x, sb.x, hb.x)); vb[i].y = act_in<XACT>(fmaf(vb[i].y, sb.y, hb.y));
+      vb[i].z = act_in<XACT>(fmaf(vb[i].z, sb.z, hb.z)); vb[i].w = act_in<XACT>(fmaf(vb[i].w, sb.w, hb.w));
+    }
+  }
+  if (rows_valid < TR) {                          // rows past the end of the tensor / of the split stay (or become) zero
+#pragma unroll
+    for (int i = 0; i < M::ROWS; ++i)
+      if (r0 + i * M::RSTEP >= rows_valid) { va[i] = make_float4(0.f, 0.f, 0.f, 0.f); vb[i] = va[i]; }
+  }
+  if (gate != nullptr && k < K) {
+    const bool k2 = k + 4 < K;
+    const float4 one = make_float4(1.f, 1.f, 1.f, 1.f);
+    if (rps >= TR) {
+      // a 128-row tile touches at most two samples: both gate vectors are requested up front (L1/L2 hits) instead of
+      // one dependent load per row
+      const float4* gp0 = reinterpret_cast<const float4*>(gate + (size_t)b0 * K + k);
+      const bool two = off0 + rows_valid > rps;
+      const float4* gp1 = two ? reinterpret_cast<const float4*>(gate + (size_t)(b0 + 1) * K + k) : gp0;
+      const float4 g0a = __ldg(gp0), g0b = k2 ? __ldg(gp0 + 1) : one, g1a = __ldg(gp1), g1b = k2 ? __ldg(gp1 + 1) : one;
+#pragma unroll
+      for (int i = 0; i < M::ROWS; ++i) {
+        const bool hi_b = off0 + r0 + i * M::RSTEP >= rps;
+        const float4 ga = hi_b ? g1a : g0a, gb = hi_b ? g1b : g0b;
+        va[i].x *= ga.x; va[i].y *= ga.y; va[i].z *= ga.z; va[i].w *= ga.w;
+        vb[i].x *= gb.x; vb[i].y *= gb.y; vb[i].z *= gb.z; vb[i].w *= gb.w;
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < M::ROWS; ++i) {
+        const int r = r0 + i * M::RSTEP;
+        if (r < rows_valid) {
+          const float4* gp = reinterpret_cast<const float4*>(gate + (size_t)((off0 + r) / rps + b0) * K + k);
+          const float4 ga = __ldg(gp), gb = k2 ? __ldg(gp + 1) : one;
+          va[i].x *= ga.x; va[i].y *= ga.y; va[i].z *= ga.z; va[i].w *= ga.w;
+          vb[i].x *= gb.x; vb[i].y *= gb.y; vb[i].z *= gb.z; vb[i].w *= gb.w;
+        }
+      }
+    }
+  }
+}
+
 // A-operand tile: optional BatchNorm affine + activation (XACT >= 0) and SE gate, rows >= rows_valid forced to zero
 template <int LG, int XACT, int TR = 128>
 __device__ __forceinline__ void fix_a(unsigned char* tile, int ft, int rows_valid, const float* s_isc, const float* s_ish,
@@ -149,6 +214,41 @@ __device__ __forceinline__ void fix_a(unsigned char* tile, int ft, int rows_vali
     *reinterpret_cast<uint4*>(tile + out_hi + i * M::STRIDE) = h;
     *reinterpret_cast<uint4*>(tile + out_lo + i * M::STRIDE) = l;
     if (LG == 1) zero_upper(tile + row_off + i * M::STRIDE, cp, x);
+  }
+}
+
+// PAIR fix-up of two landed [TR rows x 32 channels] fp32 tiles of the same rows, channels c .. c+31 (ta) and c+32 .. c+63
+// (tb): afterwards each row of ta holds the 64 bf16 hi values of the 64 channels and the same row of tb their 64 bf16 lo
+// values, channel j at logical chunk j / 8.  Each tile is then a canonical MN-major SWIZZLE_128B atom column of 64
+// channels, all hi or all lo.  The transforms are fix_a's (k: channel of this thread's first value in ta).  tb_landed =
+// false: tb holds no data (its channels lie past the tensor) and counts as zeros.  Thread layout of fix_a<2>.
+template <int XACT, int TR>
+__device__ __forceinline__ void fix_pair(unsigned char* ta, unsigned char* tb, bool tb_landed, int ft, int rows_valid,
+                                         const float* s_isc, const float* s_ish, int k, const float* gate, int off0,
+                                         int b0, int rps, int K) {
+  using M = FixMap<2, TR>;
+  const int cp = ft & 3, r0 = ft >> 2;
+  const uint32_t row_off = (uint32_t)((r0 >> 3) * 1024 + (r0 & 7) * 128);
+  const int x = r0 & 7;
+  const uint32_t out_a = row_off + ((cp ^ x) << 4), out_b = row_off + (((4 + cp) ^ x) << 4);
+  float4 va[M::ROWS], vb[M::ROWS], wa[M::ROWS], wb[M::ROWS];
+  fix_load<2, XACT, TR>(ta, ft, rows_valid, s_isc, s_ish, k, gate, off0, b0, rps, K, va, vb);
+  if (tb_landed) {
+    fix_load<2, XACT, TR>(tb, ft, rows_valid, s_isc, s_ish, k + 32, gate, off0, b0, rps, K, wa, wb);
+  } else {
+#pragma unroll
+    for (int i = 0; i < M::ROWS; ++i) { wa[i] = make_float4(0.f, 0.f, 0.f, 0.f); wb[i] = wa[i]; }
+  }
+  __syncwarp();                                   // every lane of the row has read both tiles before anyone overwrites them
+#pragma unroll
+  for (int i = 0; i < M::ROWS; ++i) {
+    uint4 h0, l0, h1, l1;
+    split8(va[i], vb[i], h0, l0);
+    split8(wa[i], wb[i], h1, l1);
+    *reinterpret_cast<uint4*>(ta + out_a + i * M::STRIDE) = h0;
+    *reinterpret_cast<uint4*>(ta + out_b + i * M::STRIDE) = h1;
+    *reinterpret_cast<uint4*>(tb + out_a + i * M::STRIDE) = l0;
+    *reinterpret_cast<uint4*>(tb + out_b + i * M::STRIDE) = l1;
   }
 }
 
