@@ -299,14 +299,15 @@ class MNEngine:
     def _dispatch(self, x, return_fmaps):
         """train(): batch-statistics forward, with a graph when a parameter or the input requires grad.  eval(): the folded
         forward without a graph, unless the input requires grad: then the saving forward on running statistics."""
-        from .autograd import mn_eval_grad_forward, mn_train_forward
+        from .autograd import mn_eval_grad_forward, mn_train_forward, mn_train_forward_fmaps
         grad_on = torch.is_grad_enabled()
         input_grad = grad_on and x.requires_grad
         needs_grad = input_grad or (grad_on and any(p.requires_grad for p in self.model.parameters()))
         with torch.cuda.device(x.device):                            # launches go to x's device, whatever is current
             if self.model.training:
                 if return_fmaps:
-                    raise NotImplementedError("return_fmaps is available in eval mode only")
+                    logits, feat, fmaps = mn_train_forward_fmaps(self, x, needs_grad)
+                    return self._squeeze(logits, feat) + (fmaps,)
                 logits, feat = mn_train_forward(self, x, needs_grad)
                 return self._squeeze(logits, feat) + (None,)
             if input_grad:
@@ -412,18 +413,19 @@ class MNEngine:
     def _new_stats(self, c, dev):
         return None if self._bn_frozen else self._zero_pool.take(2, c, dev)
 
-    def _forward_train(self, x, dropout_mask=None, frozen=False):
+    def _forward_train(self, x, dropout_mask=None, frozen=False, fmaps=False):
         """Batch-statistics forward.  Returns (logits, feat, saved) where `saved` holds the raw conv outputs
         and BatchNorm statistics needed by `_backward` (activations are recomputed from them).
         frozen: the same forward with every BatchNorm on its running statistics (no buffer update) and no dropout --
-        eval mode's forward when the input's gradient is wanted."""
+        eval mode's forward when the input's gradient is wanted.
+        fmaps: saved["fmaps"] holds the 17 feature maps (stem, blocks, last conv) as NHWC tensors [B, F, T, C]."""
         self._bn_frozen = frozen
         try:
-            return self._forward_train_impl(x, dropout_mask)
+            return self._forward_train_impl(x, dropout_mask, fmaps)
         finally:
             self._bn_frozen = False
 
-    def _forward_train_impl(self, x, dropout_mask):
+    def _forward_train_impl(self, x, dropout_mask, fmaps=False):
         L = lib()
         dev = x.device
         st = _stream()
@@ -431,7 +433,7 @@ class MNEngine:
         x = x.detach().float().contiguous()
         B, _, F, T = x.shape
         HS = ACT["hswish"]
-        S = {"x": x, "B": B, "F": F, "T": T, "blocks": [], "frozen": self._bn_frozen}
+        S = {"x": x, "B": B, "F": F, "T": T, "blocks": [], "frozen": self._bn_frozen, "fmaps": [] if fmaps else None}
         self._zero_pool = _ZeroPool()
 
         conv, bn = self.stem[0], self.stem[1]
@@ -445,9 +447,13 @@ class MNEngine:
         a = torch.empty_like(z0)
         L.bn_apply(z0.data_ptr(), sc0[0].data_ptr(), sc0[1].data_ptr(), HS, 0, a.data_ptr(), dc, B * Fi * Ti, c0, st)
         S["stem"] = dict(z=z0, sc=sc0, sv=sv0, Fo=Fi, To=Ti)
+        # the stem and block outputs are materialised anyway (each is the next stage's input): the maps are these tensors
+        keep = S["fmaps"].append if fmaps else (lambda t: None)
+        keep(a)
         for blk in self.blocks:
             a, Fi, Ti, R = self._block_train_fwd(blk, a, B, Fi, Ti)
             S["blocks"].append(R)
+            keep(a)
         logits, feat = self._head_train_fwd(a, B, Fi, Ti, S, dropout_mask)
         return logits, feat, S
 
@@ -517,6 +523,11 @@ class MNEngine:
         self._gemm(a, conv.weight, zl, M, cl, conv.in_channels, stats=stt)
         scl, svl = self._finalize(bn, stt, M, dev)
         S["last"] = dict(inp=a, z=zl, sc=scl, sv=svl, Fi=Fi, Ti=Ti)
+        if S["fmaps"] is not None:
+            # the heads apply the last BatchNorm + Hardswish on load and never store them: one pass when the map is asked for
+            al = torch.empty_like(zl)
+            L.bn_apply(zl.data_ptr(), scl[0].data_ptr(), scl[1].data_ptr(), HS, 0, al.data_ptr(), dc, M, cl, st)
+            S["fmaps"].append(al)
         if self.mha is not None:
             logits, feat, S["head"] = self._mha_fwd(zl, scl, B, Fi, Ti, save=True)
             return logits, feat
@@ -809,8 +820,12 @@ class MNEngine:
                 self._pw_bwd_ok[key] = False
         return self._pw_bwd_ok[key]
 
-    def _backward(self, S, dlogits, on_ready=None, input_grad=False, wanted=None):
+    def _backward(self, S, dlogits, on_ready=None, input_grad=False, wanted=None, dembed=None, dfmaps=None):
         """-> dict {parameter: fp32 gradient view into one flat arena} (arena returned under key None).
+        dlogits, dembed ([B, C] gradient of the embedding) and dfmaps (the 17 feature maps' gradients, [B, C, F, T] of any
+        strides, fp32 or bf16; needs a forward with fmaps=True) may each be None, as may every entry of dfmaps: the
+        gradients that are given are summed.  Without dlogits the classifier's backward is skipped and its views stay 0;
+        stages no gradient reaches are skipped as well.
         on_ready(flat, i): called after each stage with the index i of the first parameter (model.parameters() order)
         whose gradient is final -- everything from i to the end is -- so a data-parallel trainer can start reducing.
         input_grad: the input spectrogram's gradient [B, 1, F, T] fp32 is returned under key "x".  wanted: the parameters
@@ -818,16 +833,32 @@ class MNEngine:
         views hold no gradient.  A forward on running statistics (S["frozen"]) gets the backward on them."""
         self._bn_frozen = S["frozen"]
         try:
-            return self._backward_impl(S, dlogits, on_ready, input_grad, wanted)
+            return self._backward_impl(S, dlogits, on_ready, input_grad, wanted, dembed, dfmaps)
         finally:
             self._bn_frozen = False
             self._unwanted = frozenset()
 
-    def _backward_impl(self, S, dlogits, on_ready, input_grad, wanted):
-        L = lib()
-        st = _stream()
-        dev = dlogits.device
-        td, dc = self.tdtype, self.dcode
+    def _add_fmap_grad(self, dy, g, shape, dtype=None):
+        """dy (+)= g.  dy: the gradient at a map's NHWC tensor [B, F, T, C] (contiguous, `dtype`, by default the storage
+        dtype), None when no gradient reached it: then a new tensor.  g: the map's own gradient [B, C, F, T] of any
+        strides, fp32 or bf16; None when the loss does not use the map: then dy is returned as it is."""
+        if g is None:
+            return dy
+        B, F, T, C = shape
+        acc = dy is not None
+        if dy is None:
+            dy = torch.empty(B, F, T, C, device=g.device, dtype=dtype or self.tdtype)
+        codes = {torch.float32: 0, torch.bfloat16: 1}
+        lib().fmap_grad_nhwc(g.data_ptr(), codes[g.dtype], *g.stride(), dy.data_ptr(), codes[dy.dtype], B, C, F, T,
+                             int(acc), _stream())
+        return dy
+
+    def _embed_grad(self, dembed, dfeat, B, C):
+        """dfeat [B, C] fp32 (+)= dembed [B, C] (any strides); dfeat None: a new tensor"""
+        return self._add_fmap_grad(dfeat, dembed[:, :, None, None], (B, 1, 1, C), torch.float32).view(B, C)
+
+    def _backward_impl(self, S, dlogits, on_ready, input_grad, wanted, dembed=None, dfmaps=None):
+        dev = S["x"].device
         B = S["B"]
         HS = ACT["hswish"]
         self._zero_pool = _ZeroPool()
@@ -840,7 +871,8 @@ class MNEngine:
         if wanted is not None:
             wanted = {id(p) for p in wanted}
             self._unwanted = frozenset(id(G[p]) for p in params if id(p) not in wanted)
-        dlogits = dlogits.float().contiguous()
+        if dlogits is not None:
+            dlogits = dlogits.float().contiguous()
         fork = self._fork = _Fork(dev, self.fork_wgrad)
         pidx = {id(p): i for i, p in enumerate(params)}
 
@@ -853,13 +885,42 @@ class MNEngine:
         Ls = S["last"]
         P = Ls["Fi"] * Ls["Ti"]
         conv, bn = self.last[0], self.last[1]
+        cl = conv.out_channels
+        last_shape = (B, Ls["Fi"], Ls["Ti"], cl)
+        dlast = dfmaps[-1] if dfmaps is not None else None     # the last conv's activated output
         if self.mha is not None:
-            gA = self._mha_bwd(S, dlogits, G, fork)
-            done(self.model.classifier)
-            dz = self._bn_bwd(gA, None, None, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, conv.out_channels, G[bn.weight],
-                              G[bn.bias], dev)
-            return self._backward_trunk(S, G, flat, fork, done, dz, input_grad)
-        H = S["head"]
+            gA = None
+            if dlogits is not None:
+                gA = self._mha_bwd(S, dlogits, G, fork)
+                done(self.model.classifier)
+            gA = self._add_fmap_grad(gA, dlast, last_shape)
+            # the embedding is the global mean of the same activation: its gradient enters as the pool's
+            dpool = self._embed_grad(dembed, None, B, cl).mul_(1.0 / P) if dembed is not None else None
+            dz = None
+            if gA is not None or dpool is not None:
+                dz = self._bn_bwd(gA, None, dpool, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, cl, G[bn.weight], G[bn.bias],
+                                  dev)
+            return self._backward_trunk(S, G, flat, fork, done, dz, input_grad, dfmaps)
+        dfeat = None
+        if dlogits is not None:
+            dfeat = self._classifier_bwd(S["head"], dlogits, G, fork, B, dev)
+            done(self.fc1)
+        if dembed is not None:
+            dfeat = self._embed_grad(dembed, dfeat, B, cl)
+
+        # ---- last 1x1 conv (+BN+Hardswish, global average pool)
+        dpool = dfeat.mul_(1.0 / P) if dfeat is not None else None    # gradient of the spatial mean, broadcast inside the BN-backward kernels
+        gA = self._add_fmap_grad(None, dlast, last_shape)
+        dz = None
+        if gA is not None or dpool is not None:
+            dz = self._bn_bwd(gA, None, dpool, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, cl, G[bn.weight], G[bn.bias], dev)
+        return self._backward_trunk(S, G, flat, fork, done, dz, input_grad, dfmaps)
+
+    def _classifier_bwd(self, H, dlogits, G, fork, B, dev):
+        """the MLP classifier's backward -> the embedding's gradient dfeat [B, C] fp32"""
+        L = lib()
+        st = _stream()
+        HS = ACT["hswish"]
         n1, ncls, cl = self.fc1.out_features, self.fc2.out_features, self.fc1.in_features
         fork.run(lambda: self._wgrad(dlogits, H["h_pre"], G[self.fc2.weight], G[self.fc2.bias], B, ncls, n1, in_sc=H["ident"],
                                      in_act=HS, gate=H["mask"], rows_per_sample=1, g_code=0, a_code=0), dlogits)
@@ -870,18 +931,15 @@ class MNEngine:
         fork.run(lambda: self._wgrad(dpre, H["feat"], G[self.fc1.weight], G[self.fc1.bias], B, n1, cl, g_code=0, a_code=0), dpre)
         dfeat = torch.empty(B, cl, device=dev, dtype=torch.float32)
         self._gemm(dpre, self.fc1.weight, dfeat, B, cl, n1, a_code=0, c_code=0, w_trans=True)
-        done(self.fc1)
+        return dfeat
 
-        # ---- last 1x1 conv (+BN+Hardswish, global average pool)
-        dpool = dfeat.mul_(1.0 / P)      # gradient of the spatial mean, broadcast inside the BN-backward kernels
-        dz = self._bn_bwd(None, None, dpool, Ls["z"], Ls["sc"], Ls["sv"], HS, B, P, cl, G[bn.weight], G[bn.bias], dev)
-        return self._backward_trunk(S, G, flat, fork, done, dz, input_grad)
-
-    def _backward_trunk(self, S, G, flat, fork, done, dz, input_grad=False):
-        """from the gradient dz at the last 1x1 conv's output down to the stem"""
+    def _backward_trunk(self, S, G, flat, fork, done, dz, input_grad=False, dfmaps=None):
+        """from the gradient dz at the last 1x1 conv's output (None: no gradient reached it) down to the stem; dfmaps[i]
+        (None or an entry None: unused) is added to the gradient at the stem's (i = 0) or block i's output before that
+        stage's backward.  A stage no gradient reaches is skipped: its parameters' views stay 0."""
         L = lib()
         st = _stream()
-        dev = dz.device
+        dev = S["x"].device
         dc = self.dcode
         B = S["B"]
         HS = ACT["hswish"]
@@ -889,22 +947,33 @@ class MNEngine:
         P = Ls["Fi"] * Ls["Ti"]
         conv = self.last[0]
         cl = conv.out_channels
-        fork.run(lambda: self._wgrad(dz, Ls["inp"], G[conv.weight], None, B * P, cl, conv.in_channels), dz)
-        dy = torch.empty_like(Ls["inp"])
-        self._gemm(dz, conv.weight, dy, B * P, conv.in_channels, cl, w_trans=True)
+        dy = None
+        if dz is not None:
+            fork.run(lambda: self._wgrad(dz, Ls["inp"], G[conv.weight], None, B * P, cl, conv.in_channels), dz)
+            dy = torch.empty_like(Ls["inp"])
+            self._gemm(dz, conv.weight, dy, B * P, conv.in_channels, cl, w_trans=True)
         done(self.last)
 
         # ---- blocks, last to first
-        for blk, R, mod in zip(reversed(self.blocks), reversed(S["blocks"]), reversed(self._block_modules())):
-            dy = self._block_bwd(blk, R, dy, G, B)
+        n = len(self.blocks)
+        for i, (blk, R, mod) in enumerate(zip(reversed(self.blocks), reversed(S["blocks"]), reversed(self._block_modules()))):
+            if dfmaps is not None:
+                dy = self._add_fmap_grad(dy, dfmaps[n - i], (B, R["Fo"], R["To"], blk.cout))
+            if dy is not None:
+                dy = self._block_bwd(blk, R, dy, G, B)
             done(mod)
         # ---- stem
         St = S["stem"]
         conv, bn = self.stem[0], self.stem[1]
         c0 = conv.out_channels
         P0 = St["Fo"] * St["To"]
+        if dfmaps is not None:
+            dy = self._add_fmap_grad(dy, dfmaps[0], (B, St["Fo"], St["To"], c0))
         fused = self.stem_bwd_fused and dc == 0 and c0 <= 64 and c0 % 4 == 0 and conv.stride[0] in (1, 2)
-        if fused or input_grad:
+        if dy is None:                                  # no gradient reached the stem
+            if input_grad:
+                G["x"] = torch.zeros(B, 1, S["F"], S["T"], device=dev, dtype=torch.float32)
+        elif fused or input_grad:
             coef = self._bn_bwd_coef(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, P0, c0, G[bn.weight], G[bn.bias],
                                      dev, dc, None)
             wgrad = self._wanted(G[conv.weight]) is not None

@@ -416,6 +416,15 @@ int eat_stem_wgrad(const void* dz, int dtype, const float* x, float* dw, int B, 
 int eat_stem_dgrad(const void* dy, int dtype, const void* z, const float* scale, const float* shift, const float* mean,
                    const float* invstd, int act, const float* c1, const float* c2, const float* w, float* dx, int B, int F,
                    int T, int C, int stride, cudaStream_t stream);
+/* The gradient of a returned feature map into NHWC storage (the reference's return_fmaps maps, models/mn/model.py:212-230,
+ * models/dymn/model.py:157-200, in training): dst[b,f,t,c] (+)= src[b,c,f,t] in fp32 arithmetic, one rounding to
+ * dst_dtype.  src is a [B, C, F, T] tensor with element strides sB, sC, sF, sT (any of them 0: an expanded broadcast);
+ * dst is contiguous [B, F, T, C].  accumulate != 0 adds to dst, else overwrites it.  src_dtype and dst_dtype are EAT_F32
+ * or EAT_BF16 each.  A source fastest along T or F goes through a shared-memory tiled transpose, one fastest along C
+ * through a vectorised direct pass.  A bad dtype, negative sizes or strides, or a null pointer -> EAT_ERR_ARG; all checks
+ * precede any launch; B = 0 (any size 0) is a no-op. */
+int eat_fmap_grad_nhwc(const void* src, int src_dtype, long long sB, long long sC, long long sF, long long sT, void* dst,
+                       int dst_dtype, int B, int C, int F, int T, int accumulate, cudaStream_t stream);
 /* dpre = dh * mask * act'(pre), fp32 vectors (classifier Hardswish + Dropout backward). */
 int eat_act_bwd(const float* dh, const float* pre, const float* mask, int act, float* dpre, long long n,
                 cudaStream_t stream);
