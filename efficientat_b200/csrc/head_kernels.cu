@@ -91,23 +91,27 @@ __global__ void __launch_bounds__(256) freq_pool_bwd_kernel(const float* __restr
 
 __device__ __forceinline__ float att_of(float s, float eps, float hi) { return fminf(fmaxf(s, eps), hi); }
 
-// one thread per (sample, class): for each head, one walk over t gives S_a = sum a and sum a*v
-__global__ void __launch_bounds__(kAttX * kAttY) att_pool_fwd_kernel(const float* __restrict__ P, const float* __restrict__ hw,
-                                                                    float eps, float hi, float* __restrict__ out,
-                                                                    float* __restrict__ sa_out, float* __restrict__ r_out,
-                                                                    int B, int Tn, int H, int K) {
+// one thread per (sample, class): for each head, one walk over t gives S_a = sum a and sum a*v.  kLen
+// (eat_att_pool_fwd_len): sample b's walk stops at t_valid[b]
+template <bool kLen>
+__device__ __forceinline__ void att_pool_fwd_body(const float* __restrict__ P, const float* __restrict__ hw, float eps,
+                                                  float hi, float* __restrict__ out, float* __restrict__ sa_out,
+                                                  float* __restrict__ r_out, int B, int Tn, int H, int K,
+                                                  const int* __restrict__ t_valid) {
   const int k = blockIdx.x * kAttX + threadIdx.x;
   const int b = blockIdx.y * kAttY + threadIdx.y;
   if (k >= K || b >= B) return;
   const long long ld = 2LL * H * K;
   const float* base = P + (long long)b * Tn * ld + k;
+  int tb = Tn;
+  if constexpr (kLen) tb = t_valid[b];
   float acc = 0.f;
   for (int h = 0; h < H; ++h) {
     const float* pa = base + (long long)h * K;
     const float* pv = pa + (long long)H * K;
     float sa = 0.f, sav = 0.f;
 #pragma unroll 4
-    for (int t = 0; t < Tn; ++t) {
+    for (int t = 0; t < tb; ++t) {
       const float a = att_of(sigmoidf_(pa[t * ld]), eps, hi);
       sa += a;
       sav = fmaf(a, pv[t * ld], sav);
@@ -121,6 +125,20 @@ __global__ void __launch_bounds__(kAttX * kAttY) att_pool_fwd_kernel(const float
     }
   }
   out[(long long)b * K + k] = acc;
+}
+
+__global__ void __launch_bounds__(kAttX * kAttY) att_pool_fwd_kernel(const float* __restrict__ P, const float* __restrict__ hw,
+                                                                    float eps, float hi, float* __restrict__ out,
+                                                                    float* __restrict__ sa_out, float* __restrict__ r_out,
+                                                                    int B, int Tn, int H, int K) {
+  att_pool_fwd_body<false>(P, hw, eps, hi, out, sa_out, r_out, B, Tn, H, K, nullptr);
+}
+
+__global__ void __launch_bounds__(kAttX * kAttY) att_pool_fwd_len_kernel(const float* __restrict__ P,
+                                                                        const float* __restrict__ hw, float eps, float hi,
+                                                                        float* __restrict__ out, int B, int Tn, int H,
+                                                                        int K, const int* __restrict__ t_valid) {
+  att_pool_fwd_body<true>(P, hw, eps, hi, out, nullptr, nullptr, B, Tn, H, K, t_valid);
 }
 
 // dv = g a, da = g (v - r), g = dout hw / S_a; dP_att = da * sigmoid'(x) where the clamp passes (eps <= sigmoid(x) <= 1-eps,
@@ -243,6 +261,19 @@ int eat_att_pool_fwd(const float* P, const float* hw, float eps, float* out, flo
   if (P == nullptr || hw == nullptr || out == nullptr) { eat_set_error("att_pool_fwd: P, hw and out are required"); return EAT_ERR_ARG; }
   const dim3 grid((unsigned)ceil_div(K, kAttX), (unsigned)ceil_div(B, kAttY));
   att_pool_fwd_kernel<<<grid, dim3(kAttX, kAttY), 0, st>>>(P, hw, eps, 1.f - eps, out, sa, r, B, T, H, K);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int eat_att_pool_fwd_len(const float* P, const float* hw, float eps, float* out, int B, int T, int H, int K,
+                         const int* t_valid, cudaStream_t st) {
+  if (int rc = att_pool_check("att_pool_fwd_len", eps, B, T, H, K)) return rc;
+  if (B == 0) return EAT_OK;
+  if (P == nullptr || hw == nullptr || out == nullptr || t_valid == nullptr) {
+    eat_set_error("att_pool_fwd_len: P, hw, out and t_valid are required"); return EAT_ERR_ARG;
+  }
+  const dim3 grid((unsigned)ceil_div(K, kAttX), (unsigned)ceil_div(B, kAttY));
+  att_pool_fwd_len_kernel<<<grid, dim3(kAttX, kAttY), 0, st>>>(P, hw, eps, 1.f - eps, out, B, T, H, K, t_valid);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }

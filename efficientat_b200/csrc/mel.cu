@@ -63,6 +63,7 @@ struct MelParams {
   float preemph;         // 0.97
   float log_offset;      // 1e-5
   float out_add, out_div;   // (v + 4.5) / 5
+  const int* n_valid;    // [B] each clip's sample count (eat_mel_fwd_len), or null
 };
 
 // sample s of the pre-emphasised signal p (length L = N-1) extended by reflection (torch.stft center=True);
@@ -88,7 +89,9 @@ __device__ __forceinline__ void group_sync(int grp) {
   }
 }
 
-template <int M>
+// kLen: clip b is the first n_valid[b] samples of its row; its frames end at 1 + (n_valid[b] - 1) / hop, past which the
+// output is 0, and pre-emphasis and reflection use its own last sample
+template <int M, bool kLen = false>
 __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
   using S = MelShape<M>;
   constexpr int G = S::kGroupThreads, F = S::kFrames, NF = S::kNfft;
@@ -106,7 +109,17 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
   const int b = blockIdx.y;
   const int t_base = blockIdx.x * F;
   const float* __restrict__ x = p.wave + (size_t)b * p.N;
-  const int L = p.N - 1;
+  const int L = kLen ? p.n_valid[b] - 1 : p.N - 1;
+  const int Tb = kLen ? 1 + L / p.hop : p.T;
+  if constexpr (kLen) {
+    if (t_base >= Tb) {                 // the whole tile lies past the clip's frames: zeros only, nothing staged or read
+      for (int i = tid; i < p.n_mels * F; i += kThreads) {
+        const int m = i / F, t = t_base + i % F;
+        if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = 0.f;
+      }
+      return;
+    }
+  }
   const int lp = (NF - p.win_length) / 2;
 
   for (int i = tid; i < NF; i += kThreads) {
@@ -128,7 +141,7 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
   for (int round = 0; round < F / S::kGroups; ++round) {
     const int fl = round * S::kGroups + grp;   // frame index inside the CTA tile
     const int t = t_base + fl;
-    const bool live = t < p.T;                 // uniform within a group
+    const bool live = t < Tb;                  // uniform within a group
     float2 v[8];
     // ---- pass 1 (Ns = 1): window the staged samples
     if (live) {
@@ -198,9 +211,14 @@ __global__ void __launch_bounds__(kThreads) mel_kernel(MelParams p) {
   const int fo = lane & (F - 1), sub = lane / F;
   const int t = t_base + fo;
   for (int m = warp * (32 / F) + sub; m < p.n_mels; m += (kThreads / 32) * (32 / F)) {
-    if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = s_out[m * (F + 1) + fo];
+    if constexpr (kLen) {
+      if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = t < Tb ? s_out[m * (F + 1) + fo] : 0.f;
+    } else {
+      if (t < p.T) p.out[((size_t)b * p.n_mels + m) * p.T + t] = s_out[m * (F + 1) + fo];
+    }
   }
 }
+
 
 template <int M>
 int mel_launch(MelParams p, cudaStream_t stream) {
@@ -211,10 +229,16 @@ int mel_launch(MelParams p, cudaStream_t stream) {
     eat_set_error("eat_mel_fwd: hop too large for the shared-memory signal slice"); return EAT_ERR_UNSUPPORTED;
   }
   p.seg_len = (int)seg_len;
-  static unsigned long long attr_mask = 0;
-  if (int rc = eat_opt_in_smem(mel_kernel<M>, kSmemCap, attr_mask)) return rc;
   dim3 grid(ceil_div(p.T, S::kFrames), p.B);
-  mel_kernel<M><<<grid, kThreads, smem, stream>>>(p);
+  if (p.n_valid == nullptr) {
+    static unsigned long long attr_mask = 0;
+    if (int rc = eat_opt_in_smem(mel_kernel<M>, kSmemCap, attr_mask)) return rc;
+    mel_kernel<M><<<grid, kThreads, smem, stream>>>(p);
+  } else {
+    static unsigned long long attr_mask_len = 0;
+    if (int rc = eat_opt_in_smem(mel_kernel<M, true>, kSmemCap, attr_mask_len)) return rc;
+    mel_kernel<M, true><<<grid, kThreads, smem, stream>>>(p);
+  }
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }
@@ -554,10 +578,11 @@ extern "C" int eat_mel_mask(float* spec, int B, int F, int T, const int* f_start
   return EAT_OK;
 }
 
-extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window, int win_length, int hop,
-                           int n_fft, const float* twiddle, const int* fb_start, const int* fb_len,
-                           const float* fb_w, int max_len, int n_mels, float preemph, float* out,
-                           cudaStream_t stream) {
+namespace {
+// n_valid: null for eat_mel_fwd; the per-clip sample counts for eat_mel_fwd_len
+int mel_fwd_impl(const float* wave, int B, int N, const float* window, int win_length, int hop, int n_fft,
+                 const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len, int n_mels,
+                 float preemph, float* out, const int* n_valid, cudaStream_t stream) {
   if (n_fft != 256 && n_fft != 512 && n_fft != 1024 && n_fft != 2048 && n_fft != 4096) {
     eat_set_error("eat_mel_fwd: n_fft must be one of 256, 512, 1024, 2048, 4096"); return EAT_ERR_UNSUPPORTED;
   }
@@ -571,6 +596,7 @@ extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window,
   p.fb_start = fb_start; p.fb_len = fb_len; p.fb_w = fb_w; p.out = out;
   p.B = B; p.N = N; p.T = 1 + (N - 1) / hop; p.n_mels = n_mels; p.win_length = win_length; p.hop = hop;
   p.max_len = max_len; p.preemph = preemph; p.log_offset = 1e-5f; p.out_add = 4.5f; p.out_div = 5.f;
+  p.n_valid = n_valid;
   switch (n_fft) {
     case 256: return mel_launch<128>(p, stream);
     case 512: return mel_launch<256>(p, stream);
@@ -578,6 +604,24 @@ extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window,
     case 2048: return mel_launch<1024>(p, stream);
     default: return mel_launch<2048>(p, stream);
   }
+}
+}  // namespace
+
+extern "C" int eat_mel_fwd(const float* wave, int B, int N, const float* window, int win_length, int hop,
+                           int n_fft, const float* twiddle, const int* fb_start, const int* fb_len,
+                           const float* fb_w, int max_len, int n_mels, float preemph, float* out,
+                           cudaStream_t stream) {
+  return mel_fwd_impl(wave, B, N, window, win_length, hop, n_fft, twiddle, fb_start, fb_len, fb_w, max_len, n_mels,
+                      preemph, out, nullptr, stream);
+}
+
+extern "C" int eat_mel_fwd_len(const float* wave, int B, int N, const float* window, int win_length, int hop,
+                               int n_fft, const float* twiddle, const int* fb_start, const int* fb_len,
+                               const float* fb_w, int max_len, int n_mels, float preemph, float* out, const int* n_valid,
+                               cudaStream_t stream) {
+  if (B > 0 && n_valid == nullptr) { eat_set_error("eat_mel_fwd_len: n_valid is required"); return EAT_ERR_ARG; }
+  return mel_fwd_impl(wave, B, N, window, win_length, hop, n_fft, twiddle, fb_start, fb_len, fb_w, max_len, n_mels,
+                      preemph, out, n_valid, stream);
 }
 
 namespace {

@@ -287,16 +287,31 @@ class MNEngine:
         return wt
 
     # ------------------------------------------------------------------ forward
-    def forward(self, x, return_fmaps=False):
+    def forward(self, x, return_fmaps=False, lengths=None):
         if not x.is_cuda:
             raise RuntimeError("efficientat_b200 models run on CUDA (sm_90a) only; got a CPU tensor")
         if x.dim() != 4 or x.shape[1] != 1:
             raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
+        lengths = self._check_lengths(x, return_fmaps, lengths)
         check_module_tensors(self.model, x.device, type(self.model).__name__)
         self.dropout_p = head_dropout(self.model)                    # read at call time (it may be changed after engine())
-        return self._dispatch(x, return_fmaps)
+        return self._dispatch(x, return_fmaps, lengths)
 
-    def _dispatch(self, x, return_fmaps):
+    def _check_lengths(self, x, return_fmaps, lengths):
+        """`lengths` (clip b is x[b, :, :, :lengths[b]]) -> list of ints, or None.  The eval forward only: in training,
+        BatchNorm's batch statistics would need the valid positions alone, which is a different semantics."""
+        if lengths is None:
+            return None
+        from .packed import check_lengths
+        if self.model.training:
+            raise NotImplementedError("lengths: per-clip lengths are supported in eval() only")
+        if x.requires_grad:
+            raise NotImplementedError("lengths: per-clip lengths are not supported for an input that requires grad")
+        if return_fmaps:
+            raise NotImplementedError("lengths: return_fmaps is not supported with per-clip lengths")
+        return check_lengths(lengths, x.shape[0], 1, x.shape[3])
+
+    def _dispatch(self, x, return_fmaps, lengths=None):
         """train(): batch-statistics forward, with a graph when a parameter or the input requires grad.  eval(): the folded
         forward without a graph, unless the input requires grad: then the saving forward on running statistics."""
         from .autograd import mn_eval_grad_forward, mn_train_forward, mn_train_forward_fmaps
@@ -315,6 +330,9 @@ class MNEngine:
                     raise NotImplementedError("return_fmaps is not available when the input requires grad")
                 logits, feat = mn_eval_grad_forward(self, x)
                 return self._squeeze(logits, feat) + (None,)
+            if lengths is not None:
+                logits, feat, _ = self._forward_eval(x.detach(), lengths=lengths)
+                return self._squeeze(logits, feat) + (None,)
             logits, feat, fmaps = self._forward_eval(x.detach(), return_fmaps)
             return self._squeeze(logits, feat) + (fmaps,)
 
@@ -324,7 +342,7 @@ class MNEngine:
         # and num_classes > 1 the squeeze is a no-op, for B == 1 the unsqueeze restores [1, C].
         return logits, feat
 
-    def _forward_eval(self, x, return_fmaps=False):
+    def _forward_eval(self, x, return_fmaps=False, lengths=None):
         L = lib()
         dev = x.device
         st = _stream()
@@ -332,6 +350,9 @@ class MNEngine:
         x = x.float().contiguous()
         B, _, F, T = x.shape
         fmaps = [] if return_fmaps else None
+        lens = None
+        if lengths is not None:
+            x, lens = self._lengths_input(x, lengths)
 
         def keep(t, f, tt, c):
             if fmaps is not None:   # NHWC storage -> logical NCHW view, like the reference's fmaps
@@ -346,15 +367,32 @@ class MNEngine:
         L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), a.data_ptr(), dc, B, F, T, c0, s0, sc[0].data_ptr(),
                    sc[1].data_ptr(), ACT["hswish"], 0, 0, st)
         keep(a, Fi, Ti, c0)
-        for blk in self.blocks:
-            a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti)
+        for i, blk in enumerate(self.blocks):
+            a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
             keep(a, Fi, Ti, blk.cout)
-        logits, feat, z = self._head_eval(a, B, Fi, Ti)
+        logits, feat, z = self._head_eval(a, B, Fi, Ti, lens)
         keep(z, Fi, Ti, self.last[0].out_channels)
         return logits, feat, fmaps
 
-    def _ir_block_eval(self, blk, a, B, Fi, Ti):
-        """one InvertedResidual with folded BatchNorm: 3-4 launches (reference block_types.py:177-181)"""
+    def _lengths_input(self, x, lengths):
+        """-> (the stem's input with 0 past each clip's end, the call's StageLengths).  The stem reads its taps past a
+        clip's end as that zero padding; the caller's tensor is never written."""
+        from .packed import StageLengths
+        B, _, F, T = x.shape
+        lens = StageLengths(self, F, T, lengths, x.device)
+        if lens.padded(0):
+            x = x.clone()
+            lib().time_pad_zero(x.data_ptr(), 0, B, F, T, 1, lens.ptr(0), _stream())
+        return x, lens
+
+    def _pad_zero(self, t, B, F, T, C, lens, s):
+        """0 past each clip's end of stage s in the engine's own tensor t [B, F, T, C], before an op that mixes along time"""
+        if lens.padded(s):
+            lib().time_pad_zero(t.data_ptr(), self.dcode, B, F, T, C, lens.ptr(s), _stream())
+
+    def _ir_block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
+        """one InvertedResidual with folded BatchNorm: 3-4 launches (reference block_types.py:177-181).
+        lens: the call's StageLengths (clips of different lengths), with stage si the block's input; None otherwise."""
         L = lib()
         dev, st = a.device, _stream()
         td, dc = self.tdtype, self.dcode
@@ -366,10 +404,14 @@ class MNEngine:
                        act=blk.act)
         else:
             e = inp
+        if lens is not None:
+            self._pad_zero(e, B, Fi, Ti, blk.cexp, lens, si)
         Fo, To = _conv_out(Fi, blk.k, blk.stride, blk.dil), _conv_out(Ti, blk.k, blk.stride, blk.dil)
         d = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         sc = self._fold(blk.dw[1], dev)
-        pool = torch.zeros(B, blk.cexp, device=dev, dtype=torch.float32) if blk.se is not None else None
+        # with lengths the squeeze is not fused into the depthwise epilogue: it would count the padded positions
+        fused_pool = blk.se is not None and lens is None
+        pool = torch.zeros(B, blk.cexp, device=dev, dtype=torch.float32) if fused_pool else None
         wt = self._dw_weights(blk.dw[0], dev)
         if blk.dil > 1:
             L.dw_conv_fwd_dil(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, blk.dil,
@@ -378,7 +420,11 @@ class MNEngine:
             L.dw_conv_fwd(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, 0, 0, 0,
                           sc[0].data_ptr(), sc[1].data_ptr(), blk.act, _ptr(pool), 0, 0, st)
         gate = None
-        if blk.se is not None:
+        if blk.se is not None and lens is not None:
+            pool = torch.empty(B, blk.cexp, device=dev, dtype=torch.float32)
+            L.mean_len(d.data_ptr(), dc, pool.data_ptr(), B, Fo, To, blk.cexp, lens.ptr(si + 1), st)
+            gate, _ = self._se_gate(blk.se, pool, 1.0, B, blk.cexp, dev)
+        elif blk.se is not None:
             gate, _ = self._se_gate(blk.se, pool, 1.0 / (Fo * To), B, blk.cexp, dev)
         Mo = B * Fo * To
         o = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
@@ -386,8 +432,9 @@ class MNEngine:
                    sc=self._fold(blk.proj[1], dev), act=0, res=inp if blk.res else None)
         return o, Fo, To
 
-    def _head_eval(self, a, B, Fi, Ti):
-        """last 1x1 conv + BN + Hardswish, global average pool, classifier MLP (mn/model.py:160-166,187-194,220-221)"""
+    def _head_eval(self, a, B, Fi, Ti, lens=None):
+        """last 1x1 conv + BN + Hardswish, global average pool, classifier MLP (mn/model.py:160-166,187-194,220-221).
+        lens: the call's StageLengths; the pools then run over each clip's valid frames."""
         L = lib()
         dev, st = a.device, _stream()
         td, dc = self.tdtype, self.dcode
@@ -396,11 +443,16 @@ class MNEngine:
         M = B * Fi * Ti
         z = torch.empty(B, Fi, Ti, cl, device=dev, dtype=td)
         self._gemm(a, conv.weight, z, M, cl, conv.in_channels, sc=self._fold(bn, dev), act=ACT["hswish"])
+        t_valid = None if lens is None else lens.ptr(lens.n - 1)
         if self.mha is not None:
-            logits, feat, _ = self._mha_fwd(z, None, B, Fi, Ti, save=False)
+            logits, feat, _ = self._mha_fwd(z, None, B, Fi, Ti, save=False, t_valid=t_valid)
             return logits, feat, z
-        feat = torch.zeros(B, cl, device=dev, dtype=torch.float32)
-        L.bn_act_pool(z.data_ptr(), 0, 0, 0, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B, Fi * Ti, cl, st)
+        if t_valid is not None:
+            feat = torch.empty(B, cl, device=dev, dtype=torch.float32)
+            L.mean_len(z.data_ptr(), dc, feat.data_ptr(), B, Fi, Ti, cl, t_valid, st)
+        else:
+            feat = torch.zeros(B, cl, device=dev, dtype=torch.float32)
+            L.bn_act_pool(z.data_ptr(), 0, 0, 0, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B, Fi * Ti, cl, st)
         h = torch.empty(B, self.fc1.out_features, device=dev, dtype=torch.float32)
         self._gemm(feat, self.fc1.weight, h, B, self.fc1.out_features, cl, bias=self.fc1.bias, act=ACT["hswish"],
                    a_code=0, c_code=0)
@@ -549,10 +601,11 @@ class MNEngine:
         S["head"] = dict(feat=feat, h_pre=h_pre, mask=dropout_mask, ident=ident)
         return logits, feat
 
-    def _mha_fwd(self, z, sc, B, Fi, Ti, save):
+    def _mha_fwd(self, z, sc, B, Fi, Ti, save, t_valid=None):
         """multi-head attention pooling head (attention_pooling.py:40-56) on the last conv's output z [B, F, T, C]:
         frequency mean (with the BatchNorm + Hardswish applied on load when sc is given, i.e. z is raw), projection GEMM,
-        attention pooling.  -> (logits [B, K], features [B, C], tensors the backward needs or None)"""
+        attention pooling.  -> (logits [B, K], features [B, C], tensors the backward needs or None).
+        t_valid: device row of each clip's valid frames (eval with lengths): features and the attention sums stop there."""
         L = lib()
         dev, st = z.device, _stream()
         head = self.mha
@@ -560,11 +613,18 @@ class MNEngine:
         m = torch.empty(B, Ti, C, device=dev, dtype=torch.float32)
         feat = torch.empty(B, C, device=dev, dtype=torch.float32)
         L.freq_pool(z.data_ptr(), self.dcode, _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0,
-                    ACT["hswish"] if sc is not None else 0, m.data_ptr(), feat.data_ptr(), B, Fi, Ti, C, st)
+                    ACT["hswish"] if sc is not None else 0, m.data_ptr(), feat.data_ptr() if t_valid is None else 0, B, Fi,
+                    Ti, C, st)
+        if t_valid is not None:
+            L.mean_len(z.data_ptr(), self.dcode, feat.data_ptr(), B, Fi, Ti, C, t_valid, st)
         P = torch.empty(B * Ti, 2 * H * K, device=dev, dtype=torch.float32)
         proj = head.subspace_proj
         self._gemm(m, proj.weight, P, B * Ti, 2 * H * K, C, bias=proj.bias, a_code=0, c_code=0)
         logits = torch.empty(B, K, device=dev, dtype=torch.float32)
+        if t_valid is not None:
+            L.att_pool_fwd_len(P.data_ptr(), head.head_weight.data_ptr(), head.epsilon, logits.data_ptr(), B, Ti, H, K,
+                               t_valid, st)
+            return logits, feat, None
         sa = r = None
         if save:
             sa = torch.empty(B, H, K, device=dev, dtype=torch.float32)

@@ -46,14 +46,15 @@ class DyMNEngine(MNEngine):
     def _block_modules(self):
         return list(self.model.layers)
 
-    def forward(self, x, return_fmaps=False):
+    def forward(self, x, return_fmaps=False, lengths=None):
         if not x.is_cuda:
             raise RuntimeError("efficientat_b200 models run on CUDA (sm_90a) only; got a CPU tensor")
         if x.dim() != 4 or x.shape[1] != 1:
             raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
+        lengths = self._check_lengths(x, return_fmaps, lengths)
         check_module_tensors(self.model, x.device, type(self.model).__name__)
         self.dropout_p = float(self.model.classifier[4].p)
-        return self._dispatch(x, return_fmaps)
+        return self._dispatch(x, return_fmaps, lengths)
 
     # ------------------------------------------------------------------ DynamicConv 1x1 dispatch
     def _mixed_weights(self, W, att, B, n):
@@ -100,7 +101,8 @@ class DyMNEngine(MNEngine):
                             _stream())
 
     # ------------------------------------------------------------------
-    def _dy_block_eval(self, blk, a, B, Fi, Ti):
+    def _dy_block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
+        """lens: the call's StageLengths (clips of different lengths), with stage si the block's input; None otherwise"""
         L = lib()
         st = _stream()
         dev = a.device
@@ -112,12 +114,22 @@ class DyMNEngine(MNEngine):
         f32 = torch.float32
         # ---- ContextGen (dy_block.py:235-254)
         g = torch.empty(B, P, blk.cin, device=dev, dtype=f32)
-        L.ctx_pool(a.data_ptr(), dc, g.data_ptr(), B, Fi, Ti, blk.cin, st)
+        if lens is None:
+            L.ctx_pool(a.data_ptr(), dc, g.data_ptr(), B, Fi, Ti, blk.cin, st)
+        else:
+            L.ctx_pool_len(a.data_ptr(), dc, g.data_ptr(), B, Fi, Ti, blk.cin, lens.ptr(si), st)
         hcat = torch.empty(B * P, H, device=dev, dtype=f32)
         self._gemm(g, cg.joint_conv.weight, hcat, B * P, H, blk.cin, sc=self._fold(cg.joint_norm, dev), act=ACT["hswish"],
                    a_code=0, c_code=0)
-        h_c = torch.zeros(B, H, device=dev, dtype=f32)
-        L.bn_act_pool(hcat.data_ptr(), 0, 0, 0, h_c.data_ptr(), 1.0 / P, 0, B, P, H, st)
+        if lens is None:
+            h_c = torch.zeros(B, H, device=dev, dtype=f32)
+            L.bn_act_pool(hcat.data_ptr(), 0, 0, 0, h_c.data_ptr(), 1.0 / P, 0, B, P, H, st)
+        else:
+            # the sequence of clip b is its first Fi + t_b rows: 0 beyond them is the time AvgPool's own zero padding
+            h_c = torch.empty(B, H, device=dev, dtype=f32)
+            if lens.padded(si):
+                L.time_pad_zero(hcat.data_ptr(), 0, B, 1, P, H, lens.seq_ptr(si), st)
+            L.mean_len(hcat.data_ptr(), 0, h_c.data_ptr(), B, 1, P, H, lens.seq_ptr(si), st)
         s = blk.stride
         Fo, To = _conv_out(Fi, blk.k, s), _conv_out(Ti, blk.k, s)
         hf = torch.empty(B, Fo, H, device=dev, dtype=f32)
@@ -147,6 +159,8 @@ class DyMNEngine(MNEngine):
                            act=blk.act)
         else:
             e = inp
+        if lens is not None:
+            self._pad_zero(e, B, Fi, Ti, blk.cexp, lens, si)
         # ---- depthwise DynamicConv + BN + DyReLU-B + CoordAtt
         att = attention(m.depth_conv)
         kk = blk.k * blk.k
@@ -176,7 +190,7 @@ class DyMNEngine(MNEngine):
                        res=inp if blk.res else None)
         return o, Fo, To
 
-    def _forward_eval(self, x, return_fmaps=False):
+    def _forward_eval(self, x, return_fmaps=False, lengths=None):
         L = lib()
         dev = x.device
         st = _stream()
@@ -184,6 +198,9 @@ class DyMNEngine(MNEngine):
         x = x.float().contiguous()
         B, _, F, T = x.shape
         fmaps = [] if return_fmaps else None
+        lens = None
+        if lengths is not None:
+            x, lens = self._lengths_input(x, lengths)
 
         def keep(t, f, tt, c):
             if fmaps is not None:
@@ -198,13 +215,13 @@ class DyMNEngine(MNEngine):
         L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), a.data_ptr(), dc, B, F, T, c0, s0, sc[0].data_ptr(),
                    sc[1].data_ptr(), ACT["hswish"], 0, 0, st)
         keep(a, Fi, Ti, c0)
-        for blk in self.blocks:
+        for i, blk in enumerate(self.blocks):
             if blk.dy:
-                a, Fi, Ti = self._dy_block_eval(blk, a, B, Fi, Ti)
+                a, Fi, Ti = self._dy_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
             else:
-                a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti)
+                a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
             keep(a, Fi, Ti, blk.cout)
-        logits, feat, z = self._head_eval(a, B, Fi, Ti)
+        logits, feat, z = self._head_eval(a, B, Fi, Ti, lens)
         keep(z, Fi, Ti, self.last[0].out_channels)
         return logits, feat, fmaps
 

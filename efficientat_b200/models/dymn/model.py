@@ -68,12 +68,13 @@ class DyMN(nn.Module):
             object.__setattr__(self, "_engine", DyMNEngine(self))
         return self._engine
 
-    def _forward_impl(self, x: Tensor, return_fmaps: bool = False):
-        logits, embed, fmaps = self.engine().forward(x, return_fmaps=return_fmaps)
+    def _forward_impl(self, x: Tensor, return_fmaps: bool = False, lengths=None):
+        """lengths (eval only): each clip's frame count, as MN._forward_impl"""
+        logits, embed, fmaps = self.engine().forward(x, return_fmaps=return_fmaps, lengths=lengths)
         return (logits, fmaps) if return_fmaps else (logits, embed)
 
-    def forward(self, x: Tensor, return_fmaps: bool = False):
-        return self._forward_impl(x, return_fmaps)
+    def forward(self, x: Tensor, return_fmaps: bool = False, lengths=None):
+        return self._forward_impl(x, return_fmaps, lengths)
 
     def update_params(self, epoch):
         """per-epoch DynamicConv temperature update (ex_audioset.py:132-133)"""

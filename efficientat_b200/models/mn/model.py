@@ -86,12 +86,14 @@ class MN(nn.Module):
             object.__setattr__(self, "_engine", MNEngine(self))
         return self._engine
 
-    def _forward_impl(self, x: Tensor, return_fmaps: bool = False):
-        logits, features, fmaps = self.engine().forward(x, return_fmaps=return_fmaps)
+    def _forward_impl(self, x: Tensor, return_fmaps: bool = False, lengths=None):
+        """lengths (eval only): each clip's frame count, a sequence of ints or a CPU integer tensor of length B.  Row b
+        of the result then equals the model on x[b:b+1, :, :, :lengths[b]] alone; x past a clip's length is never used."""
+        logits, features, fmaps = self.engine().forward(x, return_fmaps=return_fmaps, lengths=lengths)
         return (logits, fmaps) if return_fmaps else (logits, features)
 
-    def forward(self, x: Tensor):
-        return self._forward_impl(x)
+    def forward(self, x: Tensor, lengths=None):
+        return self._forward_impl(x, lengths=lengths)
 
 
 def _mobilenet_v3_conf(width_mult: float = 1.0, reduced_tail: bool = False, dilated: bool = False,

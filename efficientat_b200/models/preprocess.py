@@ -11,6 +11,7 @@ import torch
 import torch.nn as nn
 
 from .._lib import check_module_tensors, lib
+from ..packed import as_int_list, check_lengths
 from .filterbank import kaldi_mel_banks, to_bands
 
 
@@ -98,19 +99,40 @@ class AugmentMelSTFT(nn.Module):
                              buf[1].data_ptr(), buf[2].data_ptr(), cap, torch.cuda.current_stream().cuda_stream)
         return buf[0], buf[1], buf[2], cap
 
-    def forward(self, x):
+    def forward(self, x, lengths=None):
+        """x [B, N] -> log-mel [B, n_mels, 1 + (N - 1) // hopsize].
+
+        lengths (eval only): each clip's sample count, a sequence of ints or a CPU integer tensor of length B, each
+        between n_fft // 2 + 2 (the shortest waveform the call accepts) and N.  Clip b's frames t < num_frames(lengths)[b]
+        then equal this module on x[b:b+1, :lengths[b]] alone (pre-emphasis and reflect padding end at the clip's own
+        last sample); later frames are 0.0; samples at or past lengths[b] are never read.  The two torch.randint draws
+        of every call happen once per call, not once per clip."""
         if not x.is_cuda:
             raise RuntimeError("efficientat_b200.AugmentMelSTFT runs on CUDA (sm_90a) only; got a CPU tensor")
         if x.dim() != 2:
             raise ValueError(f"expected waveform of shape [B, N], got {tuple(x.shape)}")
+        if lengths is not None:
+            if self.training:
+                raise NotImplementedError("lengths: per-clip lengths are supported in eval() only")
+            if x.requires_grad:
+                raise NotImplementedError("lengths: per-clip lengths are not supported for a waveform that requires grad")
+            lengths = check_lengths(lengths, x.shape[0], self.n_fft // 2 + 2, x.shape[1])
         check_module_tensors(self, x.device, "AugmentMelSTFT")
         with torch.cuda.device(x.device):
+            if lengths is not None:
+                n_valid = torch.tensor(lengths, dtype=torch.int32).to(x.device)
+                return self._forward(x.float().contiguous(), n_valid=n_valid)
             if torch.is_grad_enabled() and x.requires_grad:
                 return _MelFn.apply(self, x)
             return self._forward(x.float().contiguous())
 
-    def _forward(self, x, saved=None):
-        """saved: a dict that receives the filterbank and masks of this call, for eat_mel_bwd"""
+    def num_frames(self, lengths):
+        """each clip's frame count for sample counts `lengths`: 1 + (n - 1) // hopsize, the `lengths` the models take"""
+        return [1 + (n - 1) // self.hopsize for n in as_int_list(lengths)]
+
+    def _forward(self, x, saved=None, n_valid=None):
+        """saved: a dict that receives the filterbank and masks of this call, for eat_mel_bwd.
+        n_valid: int32 [B] on the device, each clip's sample count (eval only)"""
         # the reference draws both randints on every call, eval included (preprocess.py:45-46)
         fmin = self.fmin + torch.randint(self.fmin_aug_range, (1,)).item()
         fmax = self.fmax + self.fmax_aug_range // 2 - torch.randint(self.fmax_aug_range, (1,)).item()
@@ -124,6 +146,12 @@ class AugmentMelSTFT(nn.Module):
         b, n = x.shape
         t = 1 + (n - 1) // self.hopsize
         out = torch.empty(b, self.n_mels, t, device=x.device, dtype=torch.float32)
+        if n_valid is not None:
+            lib().mel_fwd_len(x.data_ptr(), b, n, self.window.data_ptr(), self.win_length, self.hopsize, self.n_fft,
+                              self._twiddle.data_ptr(), start.data_ptr(), length.data_ptr(), taps.data_ptr(), max_len,
+                              self.n_mels, self._preemph, out.data_ptr(), n_valid.data_ptr(),
+                              torch.cuda.current_stream().cuda_stream)
+            return out
         lib().mel_fwd(x.data_ptr(), b, n, self.window.data_ptr(), self.win_length, self.hopsize, self.n_fft,
                       self._twiddle.data_ptr(), start.data_ptr(), length.data_ptr(), taps.data_ptr(), max_len,
                       self.n_mels, self._preemph, out.data_ptr(),

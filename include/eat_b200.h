@@ -74,6 +74,15 @@ int eat_mel_fwd(const float* wave, int B, int N, const float* window, int win_le
                 const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len,
                 int n_mels, float preemph, float* out, cudaStream_t stream);
 
+/* eat_mel_fwd on clips of different lengths in one batch: clip b is wave[b, :n_valid[b]] (n_valid: B int32 on the
+ * device).  Its frames t < 1 + (n_valid[b] - 1) / hop equal eat_mel_fwd on that clip alone (pre-emphasis and reflect
+ * padding end at its own last sample; the same per-frame arithmetic); frames up to T = 1 + (N - 1) / hop are 0.
+ * Samples at or past n_valid[b] are never read.  The caller guarantees n_fft / 2 + 2 <= n_valid[b] <= N.  Checks as
+ * eat_mel_fwd, and n_valid is required when B > 0. */
+int eat_mel_fwd_len(const float* wave, int B, int N, const float* window, int win_length, int hop, int n_fft,
+                    const float* twiddle, const int* fb_start, const int* fb_len, const float* fb_w, int max_len,
+                    int n_mels, float preemph, float* out, const int* n_valid, cudaStream_t stream);
+
 /* Adjoint of eat_mel_fwd (with eat_mel_mask's bands): dspec [B, n_mels, T] fp32 -> dwave [B, N] fp32 (overwritten), the
  * gradient through the affine, the masks (zero where the forward masked), log(mel + 1e-5), the banded filterbank, the
  * power spectrum, the real FFT, the window, the overlap-add of the frames, the reflect padding and the pre-emphasis.
@@ -448,11 +457,30 @@ int eat_freq_pool_bwd(const float* dm, float mul, void* dx, int dtype, int B, in
  * backward): sa = sum_t a, r = sum_t a v / sa.  T, H, K >= 1, 0 < eps < 0.5. */
 int eat_att_pool_fwd(const float* P, const float* hw, float eps, float* out, float* sa, float* r, int B, int T, int H, int K,
                      cudaStream_t stream);
+/* eat_att_pool_fwd where sample b's sums over t stop at t_valid[b] (B int32 on the device, 1 <= t_valid[b] <= T, which
+ * the caller guarantees): clips of different lengths in one eval batch.  No saved tensors.  Checks as eat_att_pool_fwd. */
+int eat_att_pool_fwd_len(const float* P, const float* hw, float eps, float* out, int B, int T, int H, int K,
+                         const int* t_valid, cudaStream_t stream);
 /* Its backward from dout [B,K]: dP [B*T, 2*H*K] overwritten (may alias P) with dP_val = dout hw a / sa and
  * dP_att = dout hw (v - r) / sa * sigmoid'(P_att), zero where the clamp is active (torch.clamp's gradient);
  * dhw [H] += sum_{b,k} dout r; dbias [2*H*K] += sum over rows of dP (the projection's bias gradient). */
 int eat_att_pool_bwd(const float* dout, const float* P, float* dP, const float* hw, const float* sa, const float* r, float eps,
                      float* dhw, float* dbias, int B, int T, int H, int K, cudaStream_t stream);
+
+/* ---- clips of different lengths in one eval batch (csrc/packed.cu).  x is NHWC [B, F, T, C] in dtype; sample b holds
+ * its clip in t < t_valid[b] and padding beyond.  t_valid: B int32 on the device, 1 <= t_valid[b] <= T, which the caller
+ * guarantees (the values are not read on the host).  A bad dtype, B outside [0, 65535], F outside [1, 65535], T or C
+ * below 1, or a missing pointer -> EAT_ERR_ARG before any launch; B = 0 is a no-op.  No atomics: bitwise repeatable. ---- */
+
+/* x[b, f, t, c] = 0 for t >= t_valid[b], in place; nothing else is written.  One CTA per (f, b) clears that row's
+ * contiguous (T - t_valid[b]) * C padding elements: the work is proportional to the padding. */
+int eat_time_pad_zero(void* x, int dtype, int B, int F, int T, int C, const int* t_valid, cudaStream_t stream);
+/* out[b, c] (fp32, overwritten) = mean over f < F, t < t_valid[b] of x[b, f, t, c]; the padding is never read. */
+int eat_mean_len(const void* x, int dtype, float* out, int B, int F, int T, int C, const int* t_valid, cudaStream_t stream);
+/* eat_ctx_pool with the mean over time taken over t < t_valid[b]: out [B, F+T, C] fp32 = [mean over t < t_valid[b] |
+ * mean over F for t < t_valid[b], 0 beyond].  C a multiple of 4 (fp32) or 8 (bf16). */
+int eat_ctx_pool_len(const void* x, int dtype, float* out, int B, int F, int T, int C, const int* t_valid,
+                     cudaStream_t stream);
 
 /* ---- training step around the network (ex_audioset.py:135-199) ---- */
 
