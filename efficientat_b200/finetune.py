@@ -35,14 +35,14 @@ LOSSES = ("ce", "bce", "bce_masked")
 class FineTuneTrainer(AudioSetTrainer):
     def __init__(self, model, mel, loss="ce", lr=8e-4, mixup_alpha=0.3, mixstyle_p=0.0, mixstyle_alpha=0.4,
                  weight_decay=0.0, adamw=False, betas=(0.9, 0.999), eps=1e-8, process_group=None, cuda_graph=False,
-                 schedule=None, grad_buckets=3):
+                 schedule=None, grad_buckets=3, augment=None):
         if loss not in LOSSES:
             raise ValueError(f"FineTuneTrainer: loss must be one of {LOSSES}, got {loss!r}")
         if mixstyle_p and loss != "ce":
             raise ValueError("FineTuneTrainer: MixStyle is part of the cross-entropy (DCASE20) step only")
         super().__init__(model, mel, lr=lr, kd_lambda=1.0, mixup_alpha=mixup_alpha, weight_decay=weight_decay,
                          adamw=adamw, betas=betas, eps=eps, process_group=process_group, cuda_graph=cuda_graph,
-                         schedule=schedule, grad_buckets=grad_buckets)
+                         schedule=schedule, grad_buckets=grad_buckets, augment=augment)
         self.loss = loss
         self.mixstyle_p, self.mixstyle_alpha = mixstyle_p, mixstyle_alpha
 
@@ -66,10 +66,12 @@ class FineTuneTrainer(AudioSetTrainer):
             raise ValueError(f"loss='bce_masked' takes y = [B, 2C] (targets | mask), got {tuple(y.shape)}")
         return y.to(torch.float32).contiguous()
 
-    def forward_backward(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None):
+    def forward_backward(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None, draws=None):
         """-> (loss fp64 device scalar, flat gradient arena)"""
         L = lib()
         st = _stream()
+        if self.augment is not None:
+            wave, y = self.augment(wave, y, draws)
         B = wave.shape[0]
         spec = self.mel(wave.reshape(B, -1))                       # [B, n_mels, T]
         dev = spec.device
@@ -117,7 +119,9 @@ class FineTuneTrainer(AudioSetTrainer):
     def _graph_key(self, spec, y, teacher, perm_d, known):
         return super()._graph_key(spec, y, teacher, perm_d, known) + (self.loss, y.dtype)
 
-    def step(self, wave, y, perm=None, lam=None):
+    def step(self, wave, y, perm=None, lam=None, draws=None):
         """one optimiser step on a batch: wave [B, N] (or [B, 1, N]) and y as described for `loss`; perm/lam
-        optionally replace the mixup draw.  -> the loss, a 0-dim fp64 device tensor"""
-        return super().step(wave, y, None, perm, lam, None)
+        optionally replace the mixup draw.  With `augment` (augment.WaveAugment) and its store, `wave` is the batch's
+        [B] dataset indices (CPU) and `y` None; `draws` optionally replaces the augmentation's draw.
+        -> the loss, a 0-dim fp64 device tensor"""
+        return super().step(wave, y, None, perm, lam, None, draws)

@@ -117,10 +117,12 @@ class AudioSetTrainer:
     `model.update_params(e)` (DyMN temperature schedule, ex_audioset.py:132-133)."""
 
     def __init__(self, model, mel, lr=8e-4, kd_lambda=0.1, mixup_alpha=0.3, weight_decay=0.0, adamw=False,
-                 betas=(0.9, 0.999), eps=1e-8, process_group=None, cuda_graph=False, schedule=None, grad_buckets=3):
+                 betas=(0.9, 0.999), eps=1e-8, process_group=None, cuda_graph=False, schedule=None, grad_buckets=3,
+                 augment=None):
         if not 0.0 <= kd_lambda <= 1.0:
             raise AssertionError("Lambda for Knowledge Distillation must be between 0 and 1.")     # ex_audioset.py:100
         self.model, self.mel = model, mel
+        self.augment = augment                  # augment.WaveAugment: gain / roll / waveform mixing before the mel
         self.engine = model.engine()
         self.lr, self.kd_lambda, self.mixup_alpha = lr, kd_lambda, mixup_alpha
         self.weight_decay, self.adamw, self.betas, self.eps = weight_decay, adamw, betas, eps
@@ -193,12 +195,14 @@ class AudioSetTrainer:
             raise RuntimeError(f"{name} must be on {dev}, got {t.device}")
         return t.to(torch.float32).contiguous()
 
-    def forward_backward(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None):
+    def forward_backward(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None, draws=None):
         """-> (loss_acc fp64[2] device = weighted label / distillation losses, flat gradient arena).
         teacher_known: optional [B] bool/float, False/0 for clips without teacher predictions (their distillation
-        loss is zeroed, ex_audioset.py:166-178)."""
+        loss is zeroed, ex_audioset.py:166-178).  With `augment`, see `step` for `wave`, `y` and `draws`."""
         L = lib()
         st = _stream()
+        if self.augment is not None:
+            wave, y = self.augment(wave, y, draws)
         B = wave.shape[0]
         spec = self.mel(wave.reshape(B, -1))                       # [B, n_mels, T]
         dev = spec.device
@@ -313,12 +317,17 @@ class AudioSetTrainer:
         if self.flat_p.is_cuda:
             torch.cuda.synchronize(self.flat_p.device)
 
-    def step(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None):
+    def step(self, wave, y, teacher=None, perm=None, lam=None, teacher_known=None, draws=None):
+        """one optimiser step.  With `augment` (augment.WaveAugment), gain, roll and waveform mixing run first, on
+        the device: with its store, `wave` is the batch's [B] dataset indices (CPU) and `y` None; without one, `wave`
+        and `y` are the batch that is augmented.  `teacher` / `teacher_known` belong to the primary items (the
+        reference looks the teacher up by the primary index, audioset.py:96-100).  `draws` optionally replaces the
+        augmentation's host draw.  -> the loss, as `forward_backward`."""
         self.model.train()
         self.mel.train()
         self.engine.dropout_p = head_dropout(self.model)             # read at call time, not at engine construction
         with torch.cuda.device(self.flat_p.device):
-            loss_acc, flat_g = self.forward_backward(wave, y, teacher, perm, lam, teacher_known)
+            loss_acc, flat_g = self.forward_backward(wave, y, teacher, perm, lam, teacher_known, draws)
             if self.world > 1 and self.bucketer is None:
                 torch.distributed.all_reduce(flat_g, group=self.pg)        # one collective per step (sum)
             self.steps += 1

@@ -524,6 +524,39 @@ int eat_bce_masked_loss(const float* logits, const float* y, int y_stride, const
 int eat_mixstyle(const float* x, const int* perm, const float* lam, float eps, float* stats, float* out, int B, int F,
                  int T, cudaStream_t stream);
 
+/* ---- waveform augmentation of the training datasets (csrc/wave_aug.cu): gain, datasets/helpers/audiodatasets.py:45-51
+ * and esc50.py:39-44 (pydub_augment, also audioset.py:58-63, fsd50k.py:62-67, openmic.py:56-61); roll,
+ * audiodatasets.py:26-38; waveform mixing, esc50.py:47-69, dcase20.py:100-118, fsd50k.py:70-92, openmic.py:74-95,
+ * audioset.py:66-88.  The random draws are made on the host (efficientat_b200/augment.py) and passed as B-vectors on
+ * the device: idx1 (int32, the primary clip, in [0, S)), idx2 (int32, the partner clip in [0, S), or -1 for a row that
+ * is not mixed), shift1/shift2 (int32 roll shifts, any value: taken mod N), gain1/gain2 (fp32 amplitudes 10^(dB/20)),
+ * lam (fp32 mixing weight).  These values are not read on the host: an index out of range makes its output row NaN.
+ * Every check precedes any launch; B == 0 is a no-op.  No atomics: bitwise repeatable. ---- */
+
+#define EAT_LABEL_PLAIN 0     /* lam y[p] + (1 - lam) y[q] over fp32 label rows (ESC-50, FSD50K, AudioSet) */
+#define EAT_LABEL_ONEHOT 1    /* the same over one-hot rows of int32 class indices (DCASE20, dcase20.py:101-114) */
+#define EAT_LABEL_OPENMIC 2   /* rows of scores | masks (C = 2H): scores masked (> 0.5) then blended, masks max-ed
+                                 (openmic.py:84-94) */
+
+/* sums[s] (fp64, overwritten) = sum over n < N of x[s, n], x [S, N] fp32: one CTA per clip, a fixed-order sum. */
+int eat_clip_sum(const float* x, int S, int N, double* sums, cudaStream_t stream);
+/* out [B, N] fp32 (overwritten, must not alias src) from src [S, N] fp32, row b with p = idx1[b], q = idx2[b]:
+ *   q < 0:   out[b, n] = gain1[b] * src[p, (n - shift1[b]) mod N]
+ *   q >= 0:  out[b, n] = l g1 src[p, (n - shift1[b]) mod N] + (1 - l) g2 src[q, (n - shift2[b]) mod N] - c0,
+ *            l = lam[b], c0 = (l g1 sums[p] + (1 - l) g2 sums[q]) / N, which is the reference's
+ *            x = l (x1 - mean x1) + (1 - l)(x2 - mean x2), x -= mean x, with x1, x2 gained and rolled.
+ * sums: eat_clip_sum of src; may be NULL when no row is mixed (a mixed row without sums is NaN).
+ * 1 <= N <= 2^30, S >= 1, B <= 65535.  Reads each source sample once per output sample; bandwidth-bound. */
+int eat_wave_aug(const float* src, const double* sums, int S, int N, const int* idx1, const int* idx2, const int* shift1,
+                 const int* shift2, const float* gain1, const float* gain2, const float* lam, float* out, int B,
+                 cudaStream_t stream);
+/* out [B, C] fp32 (overwritten) = the labels of the rows eat_wave_aug made, rule EAT_LABEL_*: y_prob [S, C] fp32 for
+ * PLAIN and OPENMIC (C even), y_index [S] int32 class indices for ONEHOT (exactly one of the two).  A row with q < 0
+ * is row p as it is (one-hot for ONEHOT; OpenMIC's scores unmasked, as the reference returns them).  A class index
+ * outside [0, C) makes its row NaN. */
+int eat_label_mix(int rule, const float* y_prob, const int* y_index, int S, int C, const int* idx1, const int* idx2,
+                  const float* lam, int B, float* out, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
