@@ -15,6 +15,7 @@ import torch
 
 from .helpers.utils import NAME_TO_WIDTH, load_labels
 from .models.preprocess import AugmentMelSTFT
+from .resample import Resample
 
 
 def window_plan(n_samples, window, hop):
@@ -52,13 +53,22 @@ class EATagger:
         self.mel = AugmentMelSTFT(n_mels=n_mels, sr=sample_rate, win_length=window_size, hopsize=hop_size)
         self.mel.to(self.device).eval()
         self.labels = list(labels) if labels is not None else load_labels()[0]
+        self._resamplers = {}                                               # native rate -> Resample, built on first use
 
     # ------------------------------------------------------------------ device part
     @torch.no_grad()
-    def window_probabilities(self, waveform, window_size=20.0, hop_length=10.0):
+    def window_probabilities(self, waveform, window_size=20.0, hop_length=10.0, sr=None):
         """waveform: 1-D (or [1, N]) float tensor / array at `sample_rate` -> (probabilities [n_windows, classes] on the
-        device, window start samples, window length in samples)."""
+        device, window start samples, window length in samples).  sr: the waveform's own rate when it is not
+        `sample_rate`; the whole recording is then resampled on the device once (efficientat_b200.resample, the semantics
+        of scipy.signal.resample_poly) and windowed after, as librosa.core.load resamples the file before the reference
+        cuts its windows."""
         w = torch.as_tensor(waveform, dtype=torch.float32).reshape(1, -1).to(self.device)
+        if sr is not None and int(sr) != self.sample_rate:
+            rs = self._resamplers.get(int(sr))
+            if rs is None:
+                rs = self._resamplers[int(sr)] = Resample(int(sr), self.sample_rate).to(self.device)
+            w = rs(w)
         win, hop = int(window_size * self.sample_rate), int(hop_length * self.sample_rate)
         n_windows, padded = window_plan(w.shape[1], win, hop)
         w = torch.nn.functional.pad(w, (0, max(padded - w.shape[1], 0)))
@@ -71,8 +81,10 @@ class EATagger:
             probs.append(torch.sigmoid(logits.float().reshape(chunk.shape[0], -1)))
         return torch.cat(probs), [i * hop for i in range(n_windows)], win
 
-    def tag_waveform(self, waveform, window_size=20.0, hop_length=10.0, top_k=10):
-        probs, starts, win = self.window_probabilities(waveform, window_size, hop_length)
+    def tag_waveform(self, waveform, window_size=20.0, hop_length=10.0, top_k=10, sr=None):
+        """sr: the waveform's rate when it is not `sample_rate` (see window_probabilities); the window times are in
+        seconds either way"""
+        probs, starts, win = self.window_probabilities(waveform, window_size, hop_length, sr=sr)
         k = min(top_k, probs.shape[1])
         p, idx = torch.topk(probs, k, dim=1)                                # descending, as argsort(preds)[::-1][:k]
         p, idx = p.cpu().numpy(), idx.cpu().numpy()                         # the recording's only device -> host copies

@@ -557,6 +557,31 @@ int eat_wave_aug(const float* src, const double* sums, int S, int N, const int* 
 int eat_label_mix(int rule, const float* y_prob, const int* y_index, int S, int C, const int* idx1, const int* idx2,
                   const float* lam, int B, float* out, cudaStream_t stream);
 
+/* ---- polyphase resampling (csrc/resample.cu): scipy.signal.resample_poly(x, up, down) with its defaults
+ * (window ('kaiser', 5.0), padtype 'constant'), the step the reference leaves to librosa.core.load(path, sr=32000) in
+ * inference.py:45, windowed_inference.py:89 and datasets/esc50.py:115.  up / down is reduced by its gcd; h is the
+ * centred filter of 2 hl + 1 taps (hl = 10 max(up, down)), so that
+ *   y[b, m] = sum_i x[b, i] h[m down - i up + hl],  m < n_out = ceil(N up / down).
+ * The filter is designed on the host (efficientat_b200/resample.py) and passed as a polyphase table [taps][rows] fp32,
+ * tap-major over the output residue: table[k][r] = h[p + (taps - 1 - k) up] with p = (r down + offset) mod up, r < up,
+ * taps = ceil((2 hl + 1) / up), and 0 where the index passes 2 hl; offset = hl.  up, down <= EAT_RESAMPLE_MAX_RATE and
+ * taps x rows <= 43008 floats, else EAT_ERR_UNSUPPORTED; n_out other than ceil(N up / down), or beyond int32, a
+ * negative offset or a missing pointer -> EAT_ERR_ARG.  All checks precede any launch; B = 0 is a no-op.  fp32
+ * accumulation, no atomics: bitwise repeatable. ---- */
+
+#define EAT_RESAMPLE_MAX_RATE 2048
+
+/* x [B, N] fp32 -> y [B, n_out] fp32 (overwritten, must not alias x).  lengths: NULL, or B int32 on the device, each
+ * clip's sample count in [1, N] (the caller checks the range): row b's outputs m < ceil(lengths[b] up / down) then equal
+ * the resampling of x[b, :lengths[b]] alone and later outputs are 0; samples at or past lengths[b] are never read. */
+int eat_resample_poly_fwd(const float* x, int B, int N, const int* lengths, int up, int down, const float* table, int taps,
+                          int offset, float* y, int n_out, cudaStream_t stream);
+/* Adjoint of eat_resample_poly_fwd without lengths: dy [B, n_out] fp32 -> dx [B, N] fp32 (overwritten),
+ * dx[b, i] = sum_m dy[b, m] h[m down - i up + hl].  table_adj is the forward's table for the exchanged pair (down, up)
+ * over h reversed: [taps_adj][down], taps_adj = ceil((2 hl + 1) / down), rows the input residue i mod down. */
+int eat_resample_poly_bwd(const float* dy, int B, int N, int up, int down, const float* table_adj, int taps_adj,
+                          int offset, float* dx, int n_out, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
