@@ -34,9 +34,14 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _stat_ptrs(stats):
-    """(sum, sq) pointers of a statistics accumulator, or nulls when the forward runs on running statistics"""
-    return (0, 0) if stats is None else (stats[0].data_ptr(), stats[1].data_ptr())
+def _pair(t):
+    """the two row pointers of a [2, C] pair (scale / shift, sum / sum of squares, mean / invstd), or nulls for None"""
+    return (0, 0) if t is None else (t[0].data_ptr(), t[1].data_ptr())
+
+
+def _xf(sc, act):
+    """(scale, shift, act) of an input transform: a BatchNorm [2, C] and activation applied on load, or none for sc None"""
+    return _pair(sc) + (act if sc is not None else 0,)
 
 
 def _conv_out(n, k, s, d=1):
@@ -45,7 +50,28 @@ def _conv_out(n, k, s, d=1):
 
 class _Layer:
     """Plain record describing one block of the network for the launcher loops."""
-    dil = 1             # depthwise dilation (MN's dilated tail: 2)
+
+
+def _block_layer(m):
+    """_Layer of one MN or DyMN block from its config, with the sub-modules of an InvertedResidual"""
+    from .models.mn.block_types import ConcurrentSEBlock, ConvNormActivation, InvertedResidual
+    cnf = m.cnf
+    L = _Layer()
+    L.res = m.use_res_connect
+    L.act = ACT["hswish"] if cnf.use_hs else ACT["relu"]
+    L.k = cnf.kernel
+    # a dilated depthwise conv runs at stride 1 (reference block_types.py:150); dilated layers go to the
+    # eat_dw_conv_*_dil entry points, never to the fused depthwise backward or the dgrad + reduce kernel
+    L.dil = cnf.dilation
+    L.stride = 1 if L.dil > 1 else cnf.stride
+    L.cin, L.cexp, L.cout = cnf.input_channels, cnf.expanded_channels, cnf.out_channels
+    if isinstance(m, InvertedResidual):
+        convs = [s for s in m.block if isinstance(s, ConvNormActivation)]
+        ses = [s for s in m.block if isinstance(s, ConcurrentSEBlock)]
+        L.expand = convs[0] if len(convs) == 3 else None
+        L.dw, L.proj = convs[-2], convs[-1]
+        L.se = ses[0].conc_se_layers[0] if ses else None
+    return L
 
 
 # one pass instead of two over the SE blocks' expanded tensors; EAT_SE_FUSED=0 restores the two-pass route
@@ -124,12 +150,17 @@ class _Fork:
             self.keep.clear()
 
 
+# runs the weight gradients in line: outside _backward, and in it unless fork_wgrad is set
+_IN_LINE = _Fork(None, False)
+
+
 class MNEngine:
     mha = None          # the MultiHeadAttentionPooling classifier, when the model has that head instead of 'mlp' (see _plan)
     # The saving forward and its backward in eval mode (input gradients): every BatchNorm runs on its running statistics,
     # whose backward is the batch-statistics formula with c1 = c2 = 0 (see _bn_bwd_coef)
     _bn_frozen = False
     _unwanted = frozenset()     # ids of gradient views no one asked for: the launches that only fill them are skipped
+    _fork = _IN_LINE
 
     def __init__(self, model):
         self.model = model
@@ -159,42 +190,18 @@ class MNEngine:
         # fp32 storage: the stem BatchNorm's backward apply inside the stem weight gradient (eat_stem_wgrad with z)
         self.stem_bwd_fused = os.environ.get("EAT_STEM_BWD_FUSED", STEM_BWD_FUSED_DEFAULT) == "1"
         self._pw_bwd_ok = {}
-        self._fork = None
         self._se_scale = {}
         self._zero_pool = _ZeroPool()
         self._plan()
 
     # ------------------------------------------------------------------ structure
     def _plan(self):
-        from .models.mn.block_types import ConcurrentSEBlock, ConvNormActivation, InvertedResidual
+        from .models.mn.block_types import InvertedResidual
         feats = list(self.model.features)
         self.stem = feats[0]
         self.last = feats[-1]
-        self.blocks = []
-        for m in feats[1:-1]:
-            assert isinstance(m, InvertedResidual)
-            L = _Layer()
-            subs = list(m.block)
-            L.expand = L.se = None
-            i = 0
-            if len([s for s in subs if isinstance(s, ConvNormActivation)]) == 3:
-                L.expand = subs[0]
-                i = 1
-            L.dw = subs[i]
-            i += 1
-            if isinstance(subs[i], ConcurrentSEBlock):
-                L.se = subs[i].conc_se_layers[0]
-                i += 1
-            L.proj = subs[i]
-            L.res = m.use_res_connect
-            L.act = ACT["hswish"] if m.cnf.use_hs else ACT["relu"]
-            L.k = m.cnf.kernel
-            # a dilated depthwise conv runs at stride 1 (reference block_types.py:150); dilated layers go to the
-            # eat_dw_conv_*_dil entry points, never to the fused depthwise backward or the dgrad + reduce kernel
-            L.dil = m.cnf.dilation
-            L.stride = 1 if L.dil > 1 else m.cnf.stride
-            L.cin, L.cexp, L.cout = m.cnf.input_channels, m.cnf.expanded_channels, m.cnf.out_channels
-            self.blocks.append(L)
+        assert all(isinstance(m, InvertedResidual) for m in feats[1:-1])
+        self.blocks = [_block_layer(m) for m in feats[1:-1]]
         self.mha = self.model.classifier if isinstance(self.model.classifier, MultiHeadAttentionPooling) else None
         if self.mha is None:
             self.fc1 = self.model.classifier[2]
@@ -216,12 +223,9 @@ class MNEngine:
         bias: [N] used as shift with scale None."""
         a_code = self.dcode if a_code is None else a_code
         c_code = self.dcode if c_code is None else c_code
-        scale = _ptr(sc[0]) if sc is not None else 0
-        shift = _ptr(sc[1]) if sc is not None else _ptr(bias)
-        args = (a.data_ptr(), a_code, w.data_ptr(), 1 if w_trans else 0, out.data_ptr(), c_code, M, N, K,
-                _ptr(in_sc[0]) if in_sc is not None else 0, _ptr(in_sc[1]) if in_sc is not None else 0, in_act,
-                _ptr(gate), rows_per_sample, scale, shift, act, _ptr(res),
-                _ptr(stats[0]) if stats is not None else 0, _ptr(stats[1]) if stats is not None else 0, _stream())
+        scale, shift = _pair(sc) if sc is not None else (0, _ptr(bias))
+        xf = _xf(in_sc, in_act)
+        epi = (_ptr(gate), rows_per_sample, scale, shift, act, _ptr(res), *_pair(stats))
         L = lib()
         use_tc = (self.gemm_impl != "simt" and a_code == c_code and M >= self.tc_min_rows and K % 8 == 0
                   and N % 8 == 0 and act != 3 and in_act != 3)      # sigmoid epilogues (DyMN context nets) stay on CUDA cores
@@ -229,23 +233,22 @@ class MNEngine:
             # fp32 storage: TMA-fed kernel; the weights are pre-split (bf16 hi|lo rows, BN scale folded, transposed for the
             # data gradient) once per launch into this scratch, so no CTA repeats that per tile
             ws = torch.empty(N * ((K + 31) // 32) * 128, device=w.device, dtype=torch.uint8)
-            L.pw_tma_fwd(a.data_ptr(), w.data_ptr(), 1 if w_trans else 0, out.data_ptr(), M, N, K, args[9], args[10], in_act,
-                         _ptr(gate), rows_per_sample, scale, shift, act, _ptr(res), args[18], args[19], ws.data_ptr(),
+            L.pw_tma_fwd(a.data_ptr(), w.data_ptr(), int(w_trans), out.data_ptr(), M, N, K, *xf, *epi, ws.data_ptr(),
                          ws.numel(), _stream())
-        elif use_tc:
-            if w_trans:      # data gradient: feed W^T [N, K] as a K-major operand
-                wt = torch.empty(N, K, device=w.device, dtype=torch.float32)
-                L.transpose_f32(w.data_ptr(), wt.data_ptr(), K, N, _stream())
-                args = (args[0], args[1], wt.data_ptr(), 0) + args[4:]
-            L.pw_tc_fwd(*args)
-        else:
-            L.gemm_simt_fwd(*args)
+            return
+        wp, w_trans = w.data_ptr(), int(w_trans)
+        if use_tc and w_trans:      # data gradient: feed W^T [N, K] as a K-major operand
+            wt = torch.empty(N, K, device=w.device, dtype=torch.float32)
+            L.transpose_f32(wp, wt.data_ptr(), K, N, _stream())
+            wp, w_trans = wt.data_ptr(), 0
+        (L.pw_tc_fwd if use_tc else L.gemm_simt_fwd)(a.data_ptr(), a_code, wp, w_trans, out.data_ptr(), c_code, M, N, K,
+                                                     *xf, *epi, _stream())
 
     def _fold(self, bn, dev):
         c = bn.num_features
         sc = torch.empty(2, c, device=dev, dtype=torch.float32)
-        lib().bn_fold(bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(),
-                      bn.running_var.data_ptr(), bn.eps, sc[0].data_ptr(), sc[1].data_ptr(), c, _stream())
+        lib().bn_fold(bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(), bn.eps,
+                      *_pair(sc), c, _stream())
         return sc
 
     def _finalize(self, bn, stats, count, dev):
@@ -258,10 +261,9 @@ class MNEngine:
         sv = torch.empty(2, c, device=dev, dtype=torch.float32)
         mom = bn.momentum if bn.momentum is not None else 0.1
         track = bn.track_running_stats and bn.running_mean is not None
-        lib().bn_finalize(stats[0].data_ptr(), stats[1].data_ptr(), float(count), bn.weight.data_ptr(),
-                          bn.bias.data_ptr(), bn.eps, mom, _ptr(bn.running_mean) if track else 0,
-                          _ptr(bn.running_var) if track else 0, _ptr(bn.num_batches_tracked) if track else 0,
-                          sc[0].data_ptr(), sc[1].data_ptr(), sv[0].data_ptr(), sv[1].data_ptr(), c, _stream())
+        lib().bn_finalize(*_pair(stats), float(count), bn.weight.data_ptr(), bn.bias.data_ptr(), bn.eps, mom,
+                          _ptr(bn.running_mean) if track else 0, _ptr(bn.running_var) if track else 0,
+                          _ptr(bn.num_batches_tracked) if track else 0, *_pair(sc), *_pair(sv), c, _stream())
         return sc, sv
 
     def _se_gate(self, se, pool, inv_count, B, C, dev, hidden=None):
@@ -321,26 +323,16 @@ class MNEngine:
         with torch.cuda.device(x.device):                            # launches go to x's device, whatever is current
             if self.model.training:
                 if return_fmaps:
-                    logits, feat, fmaps = mn_train_forward_fmaps(self, x, needs_grad)
-                    return self._squeeze(logits, feat) + (fmaps,)
-                logits, feat = mn_train_forward(self, x, needs_grad)
-                return self._squeeze(logits, feat) + (None,)
+                    return mn_train_forward_fmaps(self, x, needs_grad)
+                return mn_train_forward(self, x, needs_grad) + (None,)
             if input_grad:
                 if return_fmaps:
                     raise NotImplementedError("return_fmaps is not available when the input requires grad")
-                logits, feat = mn_eval_grad_forward(self, x)
-                return self._squeeze(logits, feat) + (None,)
+                return mn_eval_grad_forward(self, x) + (None,)
             if lengths is not None:
                 logits, feat, _ = self._forward_eval(x.detach(), lengths=lengths)
-                return self._squeeze(logits, feat) + (None,)
-            logits, feat, fmaps = self._forward_eval(x.detach(), return_fmaps)
-            return self._squeeze(logits, feat) + (fmaps,)
-
-    @staticmethod
-    def _squeeze(logits, feat):
-        # reference: `.squeeze()` then re-add the batch dim when B == 1 (mn/model.py:220-226); for B > 1
-        # and num_classes > 1 the squeeze is a no-op, for B == 1 the unsqueeze restores [1, C].
-        return logits, feat
+                return logits, feat, None
+            return self._forward_eval(x.detach(), return_fmaps)
 
     def _forward_eval(self, x, return_fmaps=False, lengths=None):
         L = lib()
@@ -364,11 +356,10 @@ class MNEngine:
         c0 = conv.out_channels
         a = torch.empty(B, Fi, Ti, c0, device=dev, dtype=td)
         sc = self._fold(bn, dev)
-        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), a.data_ptr(), dc, B, F, T, c0, s0, sc[0].data_ptr(),
-                   sc[1].data_ptr(), ACT["hswish"], 0, 0, st)
+        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), a.data_ptr(), dc, B, F, T, c0, s0, *_pair(sc), ACT["hswish"], 0, 0, st)
         keep(a, Fi, Ti, c0)
         for i, blk in enumerate(self.blocks):
-            a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
+            a, Fi, Ti = self._block_eval(blk, a, B, Fi, Ti, lens, i + 1)
             keep(a, Fi, Ti, blk.cout)
         logits, feat, z = self._head_eval(a, B, Fi, Ti, lens)
         keep(z, Fi, Ti, self.last[0].out_channels)
@@ -390,7 +381,7 @@ class MNEngine:
         if lens.padded(s):
             lib().time_pad_zero(t.data_ptr(), self.dcode, B, F, T, C, lens.ptr(s), _stream())
 
-    def _ir_block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
+    def _block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
         """one InvertedResidual with folded BatchNorm: 3-4 launches (reference block_types.py:177-181).
         lens: the call's StageLengths (clips of different lengths), with stage si the block's input; None otherwise."""
         L = lib()
@@ -415,10 +406,10 @@ class MNEngine:
         wt = self._dw_weights(blk.dw[0], dev)
         if blk.dil > 1:
             L.dw_conv_fwd_dil(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, blk.dil,
-                              0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), blk.act, _ptr(pool), 0, 0, st)
+                              0, 0, 0, *_pair(sc), blk.act, _ptr(pool), 0, 0, st)
         else:
             L.dw_conv_fwd(e.data_ptr(), wt.data_ptr(), d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, 0, 0, 0,
-                          sc[0].data_ptr(), sc[1].data_ptr(), blk.act, _ptr(pool), 0, 0, st)
+                          *_pair(sc), blk.act, _ptr(pool), 0, 0, st)
         gate = None
         if blk.se is not None and lens is not None:
             pool = torch.empty(B, blk.cexp, device=dev, dtype=torch.float32)
@@ -494,10 +485,10 @@ class MNEngine:
         c0 = conv.out_channels
         z0 = torch.empty(B, Fi, Ti, c0, device=dev, dtype=td)
         stt = self._new_stats(c0, dev)
-        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), z0.data_ptr(), dc, B, F, T, c0, s0, 0, 0, 0, *_stat_ptrs(stt), st)
+        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), z0.data_ptr(), dc, B, F, T, c0, s0, 0, 0, 0, *_pair(stt), st)
         sc0, sv0 = self._finalize(bn, stt, B * Fi * Ti, dev)
         a = torch.empty_like(z0)
-        L.bn_apply(z0.data_ptr(), sc0[0].data_ptr(), sc0[1].data_ptr(), HS, 0, a.data_ptr(), dc, B * Fi * Ti, c0, st)
+        L.bn_apply(z0.data_ptr(), *_pair(sc0), HS, 0, a.data_ptr(), dc, B * Fi * Ti, c0, st)
         S["stem"] = dict(z=z0, sc=sc0, sv=sv0, Fo=Fi, To=Ti)
         # the stem and block outputs are materialised anyway (each is the next stage's input): the maps are these tensors
         keep = S["fmaps"].append if fmaps else (lambda t: None)
@@ -510,9 +501,6 @@ class MNEngine:
         return logits, feat, S
 
     def _block_train_fwd(self, blk, a, B, Fi, Ti):
-        return self._ir_block_train_fwd(blk, a, B, Fi, Ti)
-
-    def _ir_block_train_fwd(self, blk, a, B, Fi, Ti):
         L = lib()
         dev, st = a.device, _stream()
         td, dc = self.tdtype, self.dcode
@@ -533,22 +521,20 @@ class MNEngine:
         z2 = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         stt = self._new_stats(blk.cexp, dev)
         wt = self._dw_weights(blk.dw[0], dev)
-        xf = (_ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
-              blk.act if dw_sc is not None else 0)
+        xf = _xf(dw_sc, blk.act)
         if blk.dil > 1:
             L.dw_conv_fwd_dil(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride,
-                              blk.dil, *xf, 0, 0, 0, 0, *_stat_ptrs(stt), st)
+                              blk.dil, *xf, 0, 0, 0, 0, *_pair(stt), st)
         else:
             L.dw_conv_fwd(dw_in.data_ptr(), wt.data_ptr(), z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, *xf,
-                          0, 0, 0, 0, *_stat_ptrs(stt), st)
+                          0, 0, 0, 0, *_pair(stt), st)
         sc2, sv2 = self._finalize(blk.dw[1], stt, Mo, dev)
         R.update(z2=z2, sc2=sc2, sv2=sv2, wt=wt, Fo=Fo, To=To)
         gate = None
         if blk.se is not None:
             Sq = blk.se.fc1.out_features
             pool = torch.zeros(B, blk.cexp, device=dev, dtype=torch.float32)
-            L.bn_act_pool(z2.data_ptr(), sc2[0].data_ptr(), sc2[1].data_ptr(), blk.act, pool.data_ptr(),
-                          1.0 / (Fo * To), dc, B, Fo * To, blk.cexp, st)
+            L.bn_act_pool(z2.data_ptr(), *_pair(sc2), blk.act, pool.data_ptr(), 1.0 / (Fo * To), dc, B, Fo * To, blk.cexp, st)
             gate, hidden = self._se_gate(blk.se, pool, 1.0, B, blk.cexp, dev)
             R.update(mean=pool, gate=gate, hidden=hidden)
         z3 = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
@@ -557,8 +543,7 @@ class MNEngine:
                    rows_per_sample=Fo * To, stats=stt)
         sc3, sv3 = self._finalize(blk.proj[1], stt, Mo, dev)
         a = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
-        L.bn_apply(z3.data_ptr(), sc3[0].data_ptr(), sc3[1].data_ptr(), 0, _ptr(inp) if blk.res else 0,
-                   a.data_ptr(), dc, Mo, blk.cout, st)
+        L.bn_apply(z3.data_ptr(), *_pair(sc3), 0, _ptr(inp) if blk.res else 0, a.data_ptr(), dc, Mo, blk.cout, st)
         R.update(z3=z3, sc3=sc3, sv3=sv3)
         return a, Fo, To, R
 
@@ -578,14 +563,13 @@ class MNEngine:
         if S["fmaps"] is not None:
             # the heads apply the last BatchNorm + Hardswish on load and never store them: one pass when the map is asked for
             al = torch.empty_like(zl)
-            L.bn_apply(zl.data_ptr(), scl[0].data_ptr(), scl[1].data_ptr(), HS, 0, al.data_ptr(), dc, M, cl, st)
+            L.bn_apply(zl.data_ptr(), *_pair(scl), HS, 0, al.data_ptr(), dc, M, cl, st)
             S["fmaps"].append(al)
         if self.mha is not None:
             logits, feat, S["head"] = self._mha_fwd(zl, scl, B, Fi, Ti, save=True)
             return logits, feat
         feat = torch.zeros(B, cl, device=dev, dtype=torch.float32)
-        L.bn_act_pool(zl.data_ptr(), scl[0].data_ptr(), scl[1].data_ptr(), HS, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B,
-                      Fi * Ti, cl, st)
+        L.bn_act_pool(zl.data_ptr(), *_pair(scl), HS, feat.data_ptr(), 1.0 / (Fi * Ti), dc, B, Fi * Ti, cl, st)
         # classifier: Linear -> Hardswish -> Dropout -> Linear.  The Hardswish and the dropout mask are applied on
         # the operand load of the second GEMM (in_act + per-row gate), so only the pre-activation is stored.
         n1 = self.fc1.out_features
@@ -612,9 +596,8 @@ class MNEngine:
         C, H, K = z.shape[3], head.num_heads, head.out_dim
         m = torch.empty(B, Ti, C, device=dev, dtype=torch.float32)
         feat = torch.empty(B, C, device=dev, dtype=torch.float32)
-        L.freq_pool(z.data_ptr(), self.dcode, _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0,
-                    ACT["hswish"] if sc is not None else 0, m.data_ptr(), feat.data_ptr() if t_valid is None else 0, B, Fi,
-                    Ti, C, st)
+        L.freq_pool(z.data_ptr(), self.dcode, *_xf(sc, ACT["hswish"]), m.data_ptr(), feat.data_ptr() if t_valid is None else 0,
+                    B, Fi, Ti, C, st)
         if t_valid is not None:
             L.mean_len(z.data_ptr(), self.dcode, feat.data_ptr(), B, Fi, Ti, C, t_valid, st)
         P = torch.empty(B * Ti, 2 * H * K, device=dev, dtype=torch.float32)
@@ -676,9 +659,8 @@ class MNEngine:
             return
         g_code = self.dcode if g_code is None else g_code
         a_code = self.dcode if a_code is None else a_code
-        args = (g.data_ptr(), g_code, a.data_ptr(), a_code, dW.data_ptr(), _ptr(db), M, N, K,
-                _ptr(in_sc[0]) if in_sc is not None else 0, _ptr(in_sc[1]) if in_sc is not None else 0,
-                in_act, _ptr(gate), rows_per_sample, _stream())
+        args = (g.data_ptr(), g_code, a.data_ptr(), a_code, dW.data_ptr(), _ptr(db), M, N, K, *_xf(in_sc, in_act),
+                _ptr(gate), rows_per_sample, _stream())
         use_tc = (self.gemm_impl != "simt" and db is None and g_code == a_code and M >= self.tc_min_rows
                   and K % 8 == 0 and N % 8 == 0)
         if use_tc:
@@ -701,13 +683,12 @@ class MNEngine:
             count = float("inf")
         if sums is None:
             s = self._zero_pool.take(2, C, dev)
-            L.bn_bwd_reduce(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
-                            sv[0].data_ptr(), sv[1].data_ptr(), act, code, B, P, C, s[0].data_ptr(), s[1].data_ptr(), st)
+            L.bn_bwd_reduce(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), *_pair(sc), *_pair(sv), act, code, B, P, C,
+                            *_pair(s), st)
         else:
             s = sums
         coef = torch.empty(2, C, device=dev, dtype=torch.float32)
-        L.bn_bwd_finalize(s[0].data_ptr(), s[1].data_ptr(), count, _ptr(dgamma), _ptr(dbeta),
-                          coef[0].data_ptr(), coef[1].data_ptr(), C, st)
+        L.bn_bwd_finalize(*_pair(s), count, _ptr(dgamma), _ptr(dbeta), *_pair(coef), C, st)
         return coef
 
     def _bn_bwd(self, gA, gate, dpool, z, sc, sv, act, B, P, C, dgamma, dbeta, dev, code=None, sums=None):
@@ -719,15 +700,11 @@ class MNEngine:
 
     def _bn_bwd_apply(self, gA, gate, dpool, z, sc, sv, act, coef, B, P, C, code):
         dz = torch.empty_like(z)
-        lib().bn_bwd_apply(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), sc[0].data_ptr(), sc[1].data_ptr(),
-                           sv[0].data_ptr(), sv[1].data_ptr(), act, coef[0].data_ptr(), coef[1].data_ptr(), dz.data_ptr(),
-                           code, B, P, C, _stream())
+        lib().bn_bwd_apply(_ptr(gA), _ptr(gate), _ptr(dpool), z.data_ptr(), *_pair(sc), *_pair(sv), act, *_pair(coef),
+                           dz.data_ptr(), code, B, P, C, _stream())
         return dz
 
     def _block_bwd(self, blk, R, dy, G, B):
-        return self._ir_block_bwd(blk, R, dy, G, B)
-
-    def _ir_block_bwd(self, blk, R, dy, G, B):
         """backward of one InvertedResidual; returns the gradient w.r.t. the block input"""
         L = lib()
         st = _stream()
@@ -737,7 +714,7 @@ class MNEngine:
         Pi, Po = Fi * Ti, Fo * To
         gate = R.get("gate")
         # project: BN3 (no activation)
-        fork = self._fork if self._fork is not None else _Fork(dev, False)
+        fork = self._fork
         dp = torch.empty_like(R["z2"])
         sums2 = None                                    # BN2's backward sums, when a kernel above the depthwise took them
         if (self.proj_bwd_fused and dc == 0 and blk.se is None
@@ -746,12 +723,10 @@ class MNEngine:
             coef = self._bn_bwd_coef(dy, None, None, R["z3"], R["sc3"], R["sv3"], 0, B, Po, blk.cout,
                                      G[blk.proj[1].weight], G[blk.proj[1].bias], dev, 0, None)
             sums2 = self._zero_pool.take(2, blk.cexp, dev)
-            sc3, sv3, sc2, sv2 = R["sc3"], R["sv3"], R["sc2"], R["sv2"]
-            L.pw_proj_bwd_fused(dy.data_ptr(), R["z3"].data_ptr(), sc3[0].data_ptr(), sc3[1].data_ptr(), sv3[0].data_ptr(),
-                                sv3[1].data_ptr(), coef[0].data_ptr(), coef[1].data_ptr(), R["z2"].data_ptr(),
-                                sc2[0].data_ptr(), sc2[1].data_ptr(), sv2[0].data_ptr(), sv2[1].data_ptr(), blk.act,
-                                blk.proj[0].weight.data_ptr(), dp.data_ptr(), G[blk.proj[0].weight].data_ptr(),
-                                sums2[0].data_ptr(), sums2[1].data_ptr(), 0, B * Po, blk.cexp, blk.cout, st)
+            L.pw_proj_bwd_fused(dy.data_ptr(), R["z3"].data_ptr(), *_pair(R["sc3"]), *_pair(R["sv3"]), *_pair(coef),
+                                R["z2"].data_ptr(), *_pair(R["sc2"]), *_pair(R["sv2"]), blk.act, blk.proj[0].weight.data_ptr(),
+                                dp.data_ptr(), G[blk.proj[0].weight].data_ptr(), *_pair(sums2), 0, B * Po, blk.cexp,
+                                blk.cout, st)
         else:
             dz3 = self._bn_bwd(dy, None, None, R["z3"], R["sc3"], R["sv3"], 0, B, Po, blk.cout,
                                G[blk.proj[1].weight], G[blk.proj[1].bias], dev)
@@ -767,12 +742,11 @@ class MNEngine:
                 # ~16 pixels per slice.  Every slice writes 4 x C partial sums, so few, long slices are preferred.
                 parts = max(1, min(32, (torch.cuda.get_device_properties(dev).multi_processor_count * self.se_parts_per_sm) // B, (Po + 15) // 16))
                 part = torch.empty(parts, 4, B, blk.cexp, device=dev, dtype=torch.float32)
-                L.se_bn_bwd_reduce(dp.data_ptr(), R["z2"].data_ptr(), R["sc2"][0].data_ptr(), R["sc2"][1].data_ptr(),
-                                   R["sv2"][0].data_ptr(), blk.act, dgate.data_ptr(), part.data_ptr(), parts, dc, B, Po,
-                                   blk.cexp, st)
+                L.se_bn_bwd_reduce(dp.data_ptr(), R["z2"].data_ptr(), *_pair(R["sc2"]), R["sv2"][0].data_ptr(), blk.act,
+                                   dgate.data_ptr(), part.data_ptr(), parts, dc, B, Po, blk.cexp, st)
             else:
-                L.se_bwd_reduce(dp.data_ptr(), R["z2"].data_ptr(), R["sc2"][0].data_ptr(), R["sc2"][1].data_ptr(),
-                                blk.act, dgate.data_ptr(), dc, B, Po, blk.cexp, st)
+                L.se_bwd_reduce(dp.data_ptr(), R["z2"].data_ptr(), *_pair(R["sc2"]), blk.act, dgate.data_ptr(), dc, B, Po,
+                                blk.cexp, st)
             du2 = torch.empty(B, blk.cexp, device=dev, dtype=torch.float32)
             du1 = torch.empty(B, Sq, device=dev, dtype=torch.float32)
             dpool = torch.empty(B, blk.cexp, device=dev, dtype=torch.float32)
@@ -786,10 +760,11 @@ class MNEngine:
         if blk.se is not None and self.se_fused:
             sums2 = self._zero_pool.take(2, blk.cexp, dev)
             L.se_bn_bwd_combine(part.data_ptr(), parts, gate.data_ptr(), dpool.data_ptr(), R["sv2"][1].data_ptr(), B,
-                                blk.cexp, sums2[0].data_ptr(), sums2[1].data_ptr(), st)
+                                blk.cexp, *_pair(sums2), st)
         has_exp = blk.expand is not None
         dw_in = R["z1"] if has_exp else R["inp"]
-        sc1 = R["sc1"] if has_exp else None
+        xf = _xf(R.get("sc1"), blk.act)                 # the expand stage's BatchNorm + activation on load
+        res = _ptr(dy) if (blk.res and not has_exp) else 0
         if (self.dw_bwd_fused and dc == 0 and blk.dil == 1 and (blk.k, blk.stride) in DW_BWD_FUSED_SHAPES
                 and blk.cexp % (4 if blk.k == 3 else 2) == 0):      # the kernel's channel vector: 4 (3x3) or 2 (5x5)
             # dz2 is computed on load and never stored; one walk yields the depthwise input gradient, the depthwise
@@ -798,18 +773,13 @@ class MNEngine:
                                      G[blk.dw[1].weight], G[blk.dw[1].bias], dev, dc, sums2)
             da1 = torch.empty_like(dw_in)
             sums1 = self._zero_pool.take(2, blk.cexp, dev) if has_exp else None
-            L.dw_conv_bwd_fused(dp.data_ptr(), _ptr(gate), _ptr(dpool), R["z2"].data_ptr(), R["sc2"][0].data_ptr(),
-                                R["sc2"][1].data_ptr(), R["sv2"][0].data_ptr(), R["sv2"][1].data_ptr(), blk.act,
-                                coef[0].data_ptr(), coef[1].data_ptr(), R["wt"].data_ptr(), dw_in.data_ptr(),
-                                _ptr(sc1[0]) if has_exp else 0, _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0,
-                                _ptr(dy) if (blk.res and not has_exp) else 0, da1.data_ptr(),
-                                G[blk.dw[0].weight].data_ptr(), _ptr(R["sv1"][0]) if has_exp else 0,
-                                _ptr(R["sv1"][1]) if has_exp else 0, _ptr(sums1[0]) if has_exp else 0,
-                                _ptr(sums1[1]) if has_exp else 0, dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, st)
+            L.dw_conv_bwd_fused(dp.data_ptr(), _ptr(gate), _ptr(dpool), R["z2"].data_ptr(), *_pair(R["sc2"]),
+                                *_pair(R["sv2"]), blk.act, *_pair(coef), R["wt"].data_ptr(), dw_in.data_ptr(), *xf, res,
+                                da1.data_ptr(), G[blk.dw[0].weight].data_ptr(), *_pair(R.get("sv1")), *_pair(sums1), dc, B,
+                                Fi, Ti, blk.cexp, blk.k, blk.stride, st)
             return self._expand_bwd(blk, R, dy, G, B, da1, sums1)
         dz2 = self._bn_bwd(dp, gate, dpool, R["z2"], R["sc2"], R["sv2"], blk.act, B, Po, blk.cexp,
                            G[blk.dw[1].weight], G[blk.dw[1].bias], dev, sums=sums2)
-        xf = (_ptr(sc1[0]) if has_exp else 0, _ptr(sc1[1]) if has_exp else 0, blk.act if has_exp else 0)
         if self._wanted(G[blk.dw[0].weight]) is None:
             pass                                        # the depthwise weight's gradient was not asked for
         elif blk.dil > 1:
@@ -820,17 +790,14 @@ class MNEngine:
                                              B, Fi, Ti, blk.cexp, blk.k, blk.stride, _stream()), dz2)
         da1 = torch.empty_like(dw_in)
         sums1 = None
-        res = _ptr(dy) if (blk.res and not has_exp) else 0
         if blk.dil > 1:
             L.dw_conv_dgrad_dil(dz2.data_ptr(), R["wt"].data_ptr(), res, da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
                                 blk.stride, blk.dil, st)
         elif has_exp and self.dgrad_bnred and blk.stride == 2 and dc == 0 and blk.k in (3, 5):
             # the expand BatchNorm's reduce pass rides in the epilogue of the kernel that produces its upstream gradient
             sums1 = self._zero_pool.take(2, blk.cexp, dev)
-            L.dw_conv_dgrad_bnred(dz2.data_ptr(), R["wt"].data_ptr(), 0, da1.data_ptr(), R["z1"].data_ptr(),
-                                  R["sc1"][0].data_ptr(), R["sc1"][1].data_ptr(), R["sv1"][0].data_ptr(),
-                                  R["sv1"][1].data_ptr(), blk.act, sums1[0].data_ptr(), sums1[1].data_ptr(), dc, B, Fi, Ti,
-                                  blk.cexp, blk.k, blk.stride, st)
+            L.dw_conv_dgrad_bnred(dz2.data_ptr(), R["wt"].data_ptr(), 0, da1.data_ptr(), R["z1"].data_ptr(), *_pair(R["sc1"]),
+                                  *_pair(R["sv1"]), blk.act, *_pair(sums1), dc, B, Fi, Ti, blk.cexp, blk.k, blk.stride, st)
         else:
             # without an expand stage the depthwise input IS the block input: fold the residual gradient in
             L.dw_conv_dgrad(dz2.data_ptr(), R["wt"].data_ptr(), 0, res, da1.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
@@ -849,14 +816,12 @@ class MNEngine:
             coef = self._bn_bwd_coef(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
                                      G[blk.expand[1].weight], G[blk.expand[1].bias], dev, 0, sums1)
             dinp = torch.empty_like(R["inp"])
-            sc1, sv1 = R["sc1"], R["sv1"]
-            lib().pw_conv_bwd_fused(da1.data_ptr(), R["z1"].data_ptr(), sc1[0].data_ptr(), sc1[1].data_ptr(),
-                                    sv1[0].data_ptr(), sv1[1].data_ptr(), blk.act, coef[0].data_ptr(), coef[1].data_ptr(),
-                                    R["inp"].data_ptr(), blk.expand[0].weight.data_ptr(), _ptr(dy) if blk.res else 0,
-                                    dinp.data_ptr(), G[blk.expand[0].weight].data_ptr(), 0, B * Pi, blk.cexp, blk.cin,
-                                    _stream())
+            lib().pw_conv_bwd_fused(da1.data_ptr(), R["z1"].data_ptr(), *_pair(R["sc1"]), *_pair(R["sv1"]), blk.act,
+                                    *_pair(coef), R["inp"].data_ptr(), blk.expand[0].weight.data_ptr(),
+                                    _ptr(dy) if blk.res else 0, dinp.data_ptr(), G[blk.expand[0].weight].data_ptr(), 0,
+                                    B * Pi, blk.cexp, blk.cin, _stream())
             return dinp
-        fork = self._fork if self._fork is not None else _Fork(dev, False)
+        fork = self._fork
         dz1 = self._bn_bwd(da1, None, None, R["z1"], R["sc1"], R["sv1"], blk.act, B, Pi, blk.cexp,
                            G[blk.expand[1].weight], G[blk.expand[1].bias], dev, sums=sums1)
         fork.run(lambda: self._wgrad(dz1, R["inp"], G[blk.expand[0].weight], None, B * Pi, blk.cexp, blk.cin), dz1)
@@ -897,6 +862,7 @@ class MNEngine:
         finally:
             self._bn_frozen = False
             self._unwanted = frozenset()
+            self._fork = _IN_LINE
 
     def _add_fmap_grad(self, dy, g, shape, dtype=None):
         """dy (+)= g.  dy: the gradient at a map's NHWC tensor [B, F, T, C] (contiguous, `dtype`, by default the storage
@@ -1033,31 +999,24 @@ class MNEngine:
         if dy is None:                                  # no gradient reached the stem
             if input_grad:
                 G["x"] = torch.zeros(B, 1, S["F"], S["T"], device=dev, dtype=torch.float32)
-        elif fused or input_grad:
+        else:
             coef = self._bn_bwd_coef(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, P0, c0, G[bn.weight], G[bn.bias],
                                      dev, dc, None)
-            wgrad = self._wanted(G[conv.weight]) is not None
-            if wgrad and fused:
+            if self._wanted(G[conv.weight]) is None:
+                pass                                    # the stem weight's gradient was not asked for
+            elif fused:
                 # dz0 is computed on load in its only consumer and never stored
                 L.stem_wgrad(dy.data_ptr(), 0, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
-                             conv.stride[0], St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
-                             St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(), st)
-            elif wgrad:
+                             conv.stride[0], St["z"].data_ptr(), *_pair(St["sc"]), *_pair(St["sv"]), HS, *_pair(coef), st)
+            else:
                 dz0 = self._bn_bwd_apply(dy, None, None, St["z"], St["sc"], St["sv"], HS, coef, B, P0, c0, dc)
                 L.stem_wgrad(dz0.data_ptr(), dc, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
                              conv.stride[0], 0, 0, 0, 0, 0, 0, 0, 0, st)
             if input_grad:
                 dx = torch.empty(B, 1, S["F"], S["T"], device=dev, dtype=torch.float32)
-                L.stem_dgrad(dy.data_ptr(), dc, St["z"].data_ptr(), St["sc"][0].data_ptr(), St["sc"][1].data_ptr(),
-                             St["sv"][0].data_ptr(), St["sv"][1].data_ptr(), HS, coef[0].data_ptr(), coef[1].data_ptr(),
+                L.stem_dgrad(dy.data_ptr(), dc, St["z"].data_ptr(), *_pair(St["sc"]), *_pair(St["sv"]), HS, *_pair(coef),
                              conv.weight.data_ptr(), dx.data_ptr(), B, S["F"], S["T"], c0, conv.stride[0], st)
                 G["x"] = dx
-        else:
-            dz0 = self._bn_bwd(dy, None, None, St["z"], St["sc"], St["sv"], HS, B, St["Fo"] * St["To"], c0, G[bn.weight],
-                               G[bn.bias], dev)
-            L.stem_wgrad(dz0.data_ptr(), dc, S["x"].data_ptr(), G[conv.weight].data_ptr(), B, S["F"], S["T"], c0,
-                         conv.stride[0], 0, 0, 0, 0, 0, 0, 0, 0, st)
         fork.join()
-        self._fork = None
         G[None] = flat
         return G

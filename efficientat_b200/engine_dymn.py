@@ -9,34 +9,28 @@ the bank gradients (sum_b alpha S_b) and the attention gradients (<S_b, W_k>) fo
 reductions, the coefficient / attention / coordinate nets, and the ContextGen pooling."""
 import torch
 
-from ._lib import check_module_tensors, lib
-from .engine import ACT, MNEngine, _Layer, _conv_out, _ptr, _stat_ptrs, _stream
+from ._lib import lib
+from .engine import ACT, MNEngine, _block_layer, _conv_out, _pair, _ptr, _stream, _xf
+
+SIG = 3             # sigmoid epilogue of the context nets
 
 
 class DyMNEngine(MNEngine):
     def _plan(self):
         from .models.dymn.dy_block import DY_Block
-        from .models.mn.block_types import ConvNormActivation, InvertedResidual
+        from .models.mn.block_types import InvertedResidual
         m = self.model
         self.stem, self.last = m.in_c, m.out_c
         self.blocks = []
         for blk in m.layers:
-            L = _Layer()
+            L = _block_layer(blk)
             L.dy = isinstance(blk, DY_Block)
-            cnf = blk.cnf
-            L.act = ACT["hswish"] if cnf.use_hs else ACT["relu"]
-            L.k, L.stride = cnf.kernel, cnf.stride
-            L.cin, L.cexp, L.cout = cnf.input_channels, cnf.expanded_channels, cnf.out_channels
-            L.res = blk.use_res_connect
             if L.dy:
                 L.m = blk
-                L.has_exp = cnf.expanded_channels != cnf.input_channels
+                L.has_exp = L.cexp != L.cin
                 L.H = blk.context_dim
             else:
                 assert isinstance(blk, InvertedResidual)
-                subs = [s for s in blk.block if isinstance(s, ConvNormActivation)]
-                L.expand = subs[0] if len(subs) == 3 else None
-                L.dw, L.proj, L.se = subs[-2], subs[-1], None
             self.blocks.append(L)
         self.fc1, self.fc2 = m.classifier[2], m.classifier[5]
         self.dropout_p = m.classifier[4].p
@@ -45,16 +39,6 @@ class DyMNEngine(MNEngine):
 
     def _block_modules(self):
         return list(self.model.layers)
-
-    def forward(self, x, return_fmaps=False, lengths=None):
-        if not x.is_cuda:
-            raise RuntimeError("efficientat_b200 models run on CUDA (sm_90a) only; got a CPU tensor")
-        if x.dim() != 4 or x.shape[1] != 1:
-            raise ValueError(f"expected input of shape [B, 1, F, T], got {tuple(x.shape)}")
-        lengths = self._check_lengths(x, return_fmaps, lengths)
-        check_module_tensors(self.model, x.device, type(self.model).__name__)
-        self.dropout_p = float(self.model.classifier[4].p)
-        return self._dispatch(x, return_fmaps, lengths)
 
     # ------------------------------------------------------------------ DynamicConv 1x1 dispatch
     def _mixed_weights(self, W, att, B, n):
@@ -78,31 +62,53 @@ class DyMNEngine(MNEngine):
             # this scratch.  With few rows per sample the per-sample kernels (B * N * K floats through HBM) outweigh the
             # activations and the register-staged kernel, which mixes the L2-resident banks on the fly, is the better fit
             ws = torch.empty((M // rps) * N * ((K + 31) // 32) * 128, device=A.device, dtype=torch.uint8)
-            L.pw_tma_dyn_fwd(A.data_ptr(), W.data_ptr(), att.data_ptr(), nk, 0, C.data_ptr(), M, N, K, rps,
-                             _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0, act, _ptr(res),
-                             _ptr(stats[0]) if stats is not None else 0, _ptr(stats[1]) if stats is not None else 0,
-                             ws.data_ptr(), ws.numel(), _stream())
+            L.pw_tma_dyn_fwd(A.data_ptr(), W.data_ptr(), att.data_ptr(), nk, 0, C.data_ptr(), M, N, K, rps, *_pair(sc), act,
+                             _ptr(res), *_pair(stats), ws.data_ptr(), ws.numel(), _stream())
             return
         if self.gemm_impl != "simt":
             L.pw_tc_dyn_fwd(A.data_ptr(), dc, W.data_ptr(), att.data_ptr(), nk, C.data_ptr(), M, N, K, rps, 0, 0, 0,
-                            _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0, act, _ptr(res),
-                            _ptr(stats[0]) if stats is not None else 0, _ptr(stats[1]) if stats is not None else 0,
-                            _stream())
+                            *_pair(sc), act, _ptr(res), *_pair(stats), _stream())
             return
         B = M // rps
         Wm = self._mixed_weights(W, att, B, N * K)
         es = 4 if dc == 0 else 2
         for b in range(B):
             L.gemm_simt_fwd(A.data_ptr() + b * rps * K * es, dc, Wm.data_ptr() + 4 * b * N * K, 0,
-                            C.data_ptr() + b * rps * N * es, dc, rps, N, K, 0, 0, 0, 0, 1,
-                            _ptr(sc[0]) if sc is not None else 0, _ptr(sc[1]) if sc is not None else 0, act,
-                            (res.data_ptr() + b * rps * N * es) if res is not None else 0,
-                            _ptr(stats[0]) if stats is not None else 0, _ptr(stats[1]) if stats is not None else 0,
-                            _stream())
+                            C.data_ptr() + b * rps * N * es, dc, rps, N, K, 0, 0, 0, 0, 1, *_pair(sc), act,
+                            (res.data_ptr() + b * rps * N * es) if res is not None else 0, *_pair(stats), _stream())
 
-    # ------------------------------------------------------------------
-    def _dy_block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
+    # ------------------------------------------------------------------ ContextGen (dy_block.py:235-254)
+    def _attention(self, conv, h_c, B, H):
+        """a DynamicConv's attention over its k kernels from the context h_c [B, H] -> [B, k]"""
+        att = torch.empty(B, conv.k, device=h_c.device, dtype=torch.float32)
+        lin = conv.residuals[0]
+        lib().dyconv_att(h_c.data_ptr(), lin.weight.data_ptr(), lin.bias.data_ptr(), float(conv.temperature), att.data_ptr(),
+                         B, H, conv.k, _stream())
+        return att
+
+    def _coord_att(self, blk, hseq, scJ, B, Fi, Ti, Fo, To):
+        """the coordinate branch: the joint sequence hseq [B, Fi + Ti, H] split into its frequency and time parts, pooled
+        to the depthwise output's Fo / To (with the joint BatchNorm + Hardswish on load when scJ is given, i.e. hseq is
+        raw), and the conv_f / conv_t nets -> (hf [B, Fo, H], ht [B, To, H], ca_f [B, Fo, C], ca_t [B, To, C])"""
+        L, st = lib(), _stream()
+        dev, f32 = hseq.device, torch.float32
+        cg, H, s = blk.m.context_gen, blk.H, blk.stride
+        xf = _xf(scJ, ACT["hswish"])
+        hf = torch.empty(B, Fo, H, device=dev, dtype=f32)
+        ht = torch.empty(B, To, H, device=dev, dtype=f32)
+        L.seq_pool(hseq.data_ptr(), hf.data_ptr(), B, Fi + Ti, 0, Fi, H, s, *xf, st)
+        L.seq_pool(hseq.data_ptr(), ht.data_ptr(), B, Fi + Ti, Fi, Ti, H, s, *xf, st)
+        ca_f = torch.empty(B, Fo, blk.cexp, device=dev, dtype=f32)
+        ca_t = torch.empty(B, To, blk.cexp, device=dev, dtype=f32)
+        self._gemm(hf, cg.conv_f.weight, ca_f, B * Fo, blk.cexp, H, bias=cg.conv_f.bias, act=SIG, a_code=0, c_code=0)
+        self._gemm(ht, cg.conv_t.weight, ca_t, B * To, blk.cexp, H, bias=cg.conv_t.bias, act=SIG, a_code=0, c_code=0)
+        return hf, ht, ca_f, ca_t
+
+    # ------------------------------------------------------------------ eval
+    def _block_eval(self, blk, a, B, Fi, Ti, lens=None, si=0):
         """lens: the call's StageLengths (clips of different lengths), with stage si the block's input; None otherwise"""
+        if not blk.dy:
+            return super()._block_eval(blk, a, B, Fi, Ti, lens, si)
         L = lib()
         st = _stream()
         dev = a.device
@@ -112,7 +118,6 @@ class DyMNEngine(MNEngine):
         cg = m.context_gen
         P = Fi + Ti
         f32 = torch.float32
-        # ---- ContextGen (dy_block.py:235-254)
         g = torch.empty(B, P, blk.cin, device=dev, dtype=f32)
         if lens is None:
             L.ctx_pool(a.data_ptr(), dc, g.data_ptr(), B, Fi, Ti, blk.cin, st)
@@ -132,27 +137,12 @@ class DyMNEngine(MNEngine):
             L.mean_len(hcat.data_ptr(), 0, h_c.data_ptr(), B, 1, P, H, lens.seq_ptr(si), st)
         s = blk.stride
         Fo, To = _conv_out(Fi, blk.k, s), _conv_out(Ti, blk.k, s)
-        hf = torch.empty(B, Fo, H, device=dev, dtype=f32)
-        ht = torch.empty(B, To, H, device=dev, dtype=f32)
-        L.seq_pool(hcat.data_ptr(), hf.data_ptr(), B, P, 0, Fi, H, s, 0, 0, 0, st)
-        L.seq_pool(hcat.data_ptr(), ht.data_ptr(), B, P, Fi, Ti, H, s, 0, 0, 0, st)
-        ca_f = torch.empty(B, Fo, blk.cexp, device=dev, dtype=f32)
-        ca_t = torch.empty(B, To, blk.cexp, device=dev, dtype=f32)
-        SIG = 3
-        self._gemm(hf, cg.conv_f.weight, ca_f, B * Fo, blk.cexp, H, bias=cg.conv_f.bias, act=SIG, a_code=0, c_code=0)
-        self._gemm(ht, cg.conv_t.weight, ca_t, B * To, blk.cexp, H, bias=cg.conv_t.bias, act=SIG, a_code=0, c_code=0)
-
-        def attention(dc_mod):
-            att = torch.empty(B, dc_mod.k, device=dev, dtype=f32)
-            lin = dc_mod.residuals[0]
-            L.dyconv_att(h_c.data_ptr(), lin.weight.data_ptr(), lin.bias.data_ptr(), float(dc_mod.temperature),
-                         att.data_ptr(), B, H, dc_mod.k, st)
-            return att
+        _, _, ca_f, ca_t = self._coord_att(blk, hcat, None, B, Fi, Ti, Fo, To)
 
         # ---- expand: DynamicConv 1x1 + BN + act
         inp = a
         if blk.has_exp:
-            att = attention(m.exp_conv)
+            att = self._attention(m.exp_conv, h_c, B, H)
             sc = self._fold(m.exp_norm, dev)
             e = torch.empty(B, Fi, Ti, blk.cexp, device=dev, dtype=td)
             self._dyn_gemm(inp, m.exp_conv.weight, att, m.exp_conv.k, e, B * Fi * Ti, blk.cexp, blk.cin, Fi * Ti, sc=sc,
@@ -162,7 +152,7 @@ class DyMNEngine(MNEngine):
         if lens is not None:
             self._pad_zero(e, B, Fi, Ti, blk.cexp, lens, si)
         # ---- depthwise DynamicConv + BN + DyReLU-B + CoordAtt
-        att = attention(m.depth_conv)
+        att = self._attention(m.depth_conv, h_c, B, H)
         kk = blk.k * blk.k
         wt = torch.empty(B, kk, blk.cexp, device=dev, dtype=f32)
         L.dyconv_mix_dw(m.depth_conv.weight.data_ptr(), att.data_ptr(), wt.data_ptr(), B, blk.cexp, blk.k,
@@ -173,62 +163,21 @@ class DyMNEngine(MNEngine):
         self._gemm(h_c, coef.weight, theta, B, 2 * npc * blk.cexp, H, bias=coef.bias, act=SIG, a_code=0, c_code=0)
         sc = self._fold(m.depth_norm, dev)
         d = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
-        if npc == 2:
-            L.dw_conv_fwd_dy(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
-                             0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), theta.data_ptr(), m.depth_act.lambdas.data_ptr(),
-                             m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(), 0, 0, st)
-        else:
-            L.dw_conv_fwd_dy_m(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
-                               0, 0, 0, sc[0].data_ptr(), sc[1].data_ptr(), theta.data_ptr(),
-                               m.depth_act.lambdas.data_ptr(), m.depth_act.init_v.data_ptr(), ca_f.data_ptr(),
-                               ca_t.data_ptr(), npc, 0, 0, st)
+        L.dw_conv_fwd_dy_m(e.data_ptr(), wt.data_ptr(), kk * blk.cexp, d.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
+                           0, 0, 0, *_pair(sc), theta.data_ptr(), m.depth_act.lambdas.data_ptr(),
+                           m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(), npc, 0, 0, st)
         # ---- project: DynamicConv 1x1 + BN (+ residual)
-        att = attention(m.proj_conv)
+        att = self._attention(m.proj_conv, h_c, B, H)
         sc = self._fold(m.proj_norm, dev)
         o = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
         self._dyn_gemm(d, m.proj_conv.weight, att, m.proj_conv.k, o, B * Fo * To, blk.cout, blk.cexp, Fo * To, sc=sc,
                        res=inp if blk.res else None)
         return o, Fo, To
 
-    def _forward_eval(self, x, return_fmaps=False, lengths=None):
-        L = lib()
-        dev = x.device
-        st = _stream()
-        td, dc = self.tdtype, self.dcode
-        x = x.float().contiguous()
-        B, _, F, T = x.shape
-        fmaps = [] if return_fmaps else None
-        lens = None
-        if lengths is not None:
-            x, lens = self._lengths_input(x, lengths)
-
-        def keep(t, f, tt, c):
-            if fmaps is not None:
-                fmaps.append(t.view(B, f, tt, c).permute(0, 3, 1, 2))
-
-        conv, bn = self.stem[0], self.stem[1]
-        s0 = conv.stride[0]
-        Fi, Ti = _conv_out(F, 3, s0), _conv_out(T, 3, s0)
-        c0 = conv.out_channels
-        a = torch.empty(B, Fi, Ti, c0, device=dev, dtype=td)
-        sc = self._fold(bn, dev)
-        L.stem_fwd(x.data_ptr(), conv.weight.data_ptr(), a.data_ptr(), dc, B, F, T, c0, s0, sc[0].data_ptr(),
-                   sc[1].data_ptr(), ACT["hswish"], 0, 0, st)
-        keep(a, Fi, Ti, c0)
-        for i, blk in enumerate(self.blocks):
-            if blk.dy:
-                a, Fi, Ti = self._dy_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
-            else:
-                a, Fi, Ti = self._ir_block_eval(blk, a, B, Fi, Ti, lens, i + 1)
-            keep(a, Fi, Ti, blk.cout)
-        logits, feat, z = self._head_eval(a, B, Fi, Ti, lens)
-        keep(z, Fi, Ti, self.last[0].out_channels)
-        return logits, feat, fmaps
-
     # ------------------------------------------------------------------ training
     def _block_train_fwd(self, blk, a, B, Fi, Ti):
         if not blk.dy:
-            return self._ir_block_train_fwd(blk, a, B, Fi, Ti)
+            return super()._block_train_fwd(blk, a, B, Fi, Ti)
         L = lib()
         st = _stream()
         dev = a.device
@@ -236,7 +185,7 @@ class DyMNEngine(MNEngine):
         f32 = torch.float32
         m, H, cg = blk.m, blk.H, blk.m.context_gen
         P = Fi + Ti
-        HS, SIG = ACT["hswish"], 3
+        HS = ACT["hswish"]
         R = {"inp": a, "Fi": Fi, "Ti": Ti}
         inp = a
         # ---- ContextGen with batch-statistics BatchNorm on the joint sequence
@@ -247,29 +196,15 @@ class DyMNEngine(MNEngine):
         self._gemm(g, cg.joint_conv.weight, hraw, B * P, H, blk.cin, stats=stt, a_code=0, c_code=0)
         scJ, svJ = self._finalize(cg.joint_norm, stt, B * P, dev)
         h_c = torch.zeros(B, H, device=dev, dtype=f32)
-        L.bn_act_pool(hraw.data_ptr(), scJ[0].data_ptr(), scJ[1].data_ptr(), HS, h_c.data_ptr(), 1.0 / P, 0, B, P, H, st)
+        L.bn_act_pool(hraw.data_ptr(), *_pair(scJ), HS, h_c.data_ptr(), 1.0 / P, 0, B, P, H, st)
         s = blk.stride
         Fo, To = _conv_out(Fi, blk.k, s), _conv_out(Ti, blk.k, s)
-        hf = torch.empty(B, Fo, H, device=dev, dtype=f32)
-        ht = torch.empty(B, To, H, device=dev, dtype=f32)
-        L.seq_pool(hraw.data_ptr(), hf.data_ptr(), B, P, 0, Fi, H, s, scJ[0].data_ptr(), scJ[1].data_ptr(), HS, st)
-        L.seq_pool(hraw.data_ptr(), ht.data_ptr(), B, P, Fi, Ti, H, s, scJ[0].data_ptr(), scJ[1].data_ptr(), HS, st)
-        ca_f = torch.empty(B, Fo, blk.cexp, device=dev, dtype=f32)
-        ca_t = torch.empty(B, To, blk.cexp, device=dev, dtype=f32)
-        self._gemm(hf, cg.conv_f.weight, ca_f, B * Fo, blk.cexp, H, bias=cg.conv_f.bias, act=SIG, a_code=0, c_code=0)
-        self._gemm(ht, cg.conv_t.weight, ca_t, B * To, blk.cexp, H, bias=cg.conv_t.bias, act=SIG, a_code=0, c_code=0)
+        hf, ht, ca_f, ca_t = self._coord_att(blk, hraw, scJ, B, Fi, Ti, Fo, To)
         R.update(g=g, hraw=hraw, scJ=scJ, svJ=svJ, h_c=h_c, hf=hf, ht=ht, ca_f=ca_f, ca_t=ca_t, Fo=Fo, To=To)
-
-        def attention(dc_mod):
-            att = torch.empty(B, dc_mod.k, device=dev, dtype=f32)
-            lin = dc_mod.residuals[0]
-            L.dyconv_att(h_c.data_ptr(), lin.weight.data_ptr(), lin.bias.data_ptr(), float(dc_mod.temperature),
-                         att.data_ptr(), B, H, dc_mod.k, st)
-            return att
 
         M = B * Fi * Ti
         if blk.has_exp:
-            att_e = attention(m.exp_conv)
+            att_e = self._attention(m.exp_conv, h_c, B, H)
             z1 = torch.empty(B, Fi, Ti, blk.cexp, device=dev, dtype=td)
             stt = self._new_stats(blk.cexp, dev)
             self._dyn_gemm(inp, m.exp_conv.weight, att_e, m.exp_conv.k, z1, M, blk.cexp, blk.cin, Fi * Ti, stats=stt)
@@ -278,7 +213,7 @@ class DyMNEngine(MNEngine):
             dw_in, dw_sc = z1, sc1
         else:
             dw_in, dw_sc = inp, None
-        att_d = attention(m.depth_conv)
+        att_d = self._attention(m.depth_conv, h_c, B, H)
         kk = blk.k * blk.k
         wt = torch.empty(B, kk, blk.cexp, device=dev, dtype=f32)
         L.dyconv_mix_dw(m.depth_conv.weight.data_ptr(), att_d.data_ptr(), wt.data_ptr(), B, blk.cexp, blk.k,
@@ -290,30 +225,19 @@ class DyMNEngine(MNEngine):
         Mo = B * Fo * To
         z2 = torch.empty(B, Fo, To, blk.cexp, device=dev, dtype=td)
         stt = self._new_stats(blk.cexp, dev)
-        xs = (_ptr(dw_sc[0]) if dw_sc is not None else 0, _ptr(dw_sc[1]) if dw_sc is not None else 0,
-              blk.act if dw_sc is not None else 0)
-        if npc == 2:
-            L.dw_conv_fwd_dy(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k,
-                             s, *xs, 0, 0, 0, 0, 0, 0, 0, *_stat_ptrs(stt), st)
-        else:
-            L.dw_conv_fwd_dy_m(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp,
-                               blk.k, s, *xs, 0, 0, 0, 0, 0, 0, 0, npc, *_stat_ptrs(stt), st)
+        L.dw_conv_fwd_dy_m(dw_in.data_ptr(), wt.data_ptr(), kk * blk.cexp, z2.data_ptr(), dc, B, Fi, Ti, blk.cexp, blk.k, s,
+                           *_xf(dw_sc, blk.act), 0, 0, 0, 0, 0, 0, 0, npc, *_pair(stt), st)
         sc2, sv2 = self._finalize(m.depth_norm, stt, Mo, dev)
         p = torch.empty_like(z2)
-        act_args = (z2.data_ptr(), p.data_ptr(), dc, sc2[0].data_ptr(), sc2[1].data_ptr(), theta.data_ptr(),
-                    m.depth_act.lambdas.data_ptr(), m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr())
-        if npc == 2:
-            L.dy_act_fwd(*act_args, B, Fo, To, blk.cexp, st)
-        else:
-            L.dy_act_fwd_m(*act_args, npc, B, Fo, To, blk.cexp, st)
-        att_p = attention(m.proj_conv)
+        L.dy_act_fwd_m(z2.data_ptr(), p.data_ptr(), dc, *_pair(sc2), theta.data_ptr(), m.depth_act.lambdas.data_ptr(),
+                       m.depth_act.init_v.data_ptr(), ca_f.data_ptr(), ca_t.data_ptr(), npc, B, Fo, To, blk.cexp, st)
+        att_p = self._attention(m.proj_conv, h_c, B, H)
         z3 = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
         stt = self._new_stats(blk.cout, dev)
         self._dyn_gemm(p, m.proj_conv.weight, att_p, m.proj_conv.k, z3, Mo, blk.cout, blk.cexp, Fo * To, stats=stt)
         sc3, sv3 = self._finalize(m.proj_norm, stt, Mo, dev)
         out = torch.empty(B, Fo, To, blk.cout, device=dev, dtype=td)
-        L.bn_apply(z3.data_ptr(), sc3[0].data_ptr(), sc3[1].data_ptr(), 0, _ptr(inp) if blk.res else 0, out.data_ptr(),
-                   dc, Mo, blk.cout, st)
+        L.bn_apply(z3.data_ptr(), *_pair(sc3), 0, _ptr(inp) if blk.res else 0, out.data_ptr(), dc, Mo, blk.cout, st)
         R.update(att_d=att_d, wt=wt, theta=theta, z2=z2, sc2=sc2, sv2=sv2, p=p, att_p=att_p, z3=z3, sc3=sc3, sv3=sv3,
                  dw_in=dw_in, dw_sc=dw_sc)
         return out, Fo, To, R
@@ -329,28 +253,21 @@ class DyMNEngine(MNEngine):
         W = conv.weight
         if self.gemm_impl == "simt":
             return self._dyn1x1_bwd_exact(conv, Gt, X, att, B, rps, N, K, G, res)
+        dX = torch.empty(M, K, device=dev, dtype=self.tdtype)
         if dc == 0 and self.pw_impl == "tma" and rps >= self.dyn_tma_min_rps:
             # data gradient dX_b = G_b . W_b: the same dynamic GEMM with the banks read transposed (no W^T copies)
-            dX = torch.empty(M, K, device=dev, dtype=self.tdtype)
             ws = torch.empty(B * K * ((N + 31) // 32) * 128, device=dev, dtype=torch.uint8)
             L.pw_tma_dyn_fwd(Gt.data_ptr(), W.data_ptr(), att.data_ptr(), nb, 1, dX.data_ptr(), M, K, N, rps, 0, 0, 0, _ptr(res),
                              0, 0, ws.data_ptr(), ws.numel(), st)
-            S = torch.zeros(B, N * K, device=dev, dtype=torch.float32)             # per-sample weight gradients
-            L.pw_tc_wgrad_persample(Gt.data_ptr(), X.data_ptr(), dc, S.data_ptr(), M, N, K, rps, st)
-            datt = torch.empty(B, nb, device=dev, dtype=torch.float32)
-            L.dyn_wgrad_mix(S.data_ptr(), att.data_ptr(), W.data_ptr(), G[W].data_ptr(), datt.data_ptr(), B, N * K, nb, st)
-            return dX, datt
-        Wt = torch.empty(nb, K, N, device=dev, dtype=torch.float32)           # W_k^T banks for the data gradient
-        for j in range(nb):
-            L.transpose_f32(W.data_ptr() + 4 * j * N * K, Wt.data_ptr() + 4 * j * N * K, N, K, st)
-        dX = torch.empty(M, K, device=dev, dtype=self.tdtype)
-        L.pw_tc_dyn_fwd(Gt.data_ptr(), dc, Wt.data_ptr(), att.data_ptr(), nb, dX.data_ptr(), M, K, N, rps, 0, 0, 0, 0, 0, 0,
-                        _ptr(res), 0, 0, st)
+        else:
+            Wt = torch.empty(nb, K, N, device=dev, dtype=torch.float32)           # W_k^T banks for the data gradient
+            for j in range(nb):
+                L.transpose_f32(W.data_ptr() + 4 * j * N * K, Wt.data_ptr() + 4 * j * N * K, N, K, st)
+            L.pw_tc_dyn_fwd(Gt.data_ptr(), dc, Wt.data_ptr(), att.data_ptr(), nb, dX.data_ptr(), M, K, N, rps, 0, 0, 0, 0, 0,
+                            0, _ptr(res), 0, 0, st)
         S = torch.zeros(B, N * K, device=dev, dtype=torch.float32)             # per-sample weight gradients
         L.pw_tc_wgrad_persample(Gt.data_ptr(), X.data_ptr(), dc, S.data_ptr(), M, N, K, rps, st)
-        datt = torch.empty(B, nb, device=dev, dtype=torch.float32)
-        L.dyn_wgrad_mix(S.data_ptr(), att.data_ptr(), W.data_ptr(), G[W].data_ptr(), datt.data_ptr(), B, N * K, nb, st)
-        return dX, datt
+        return dX, self._wgrad_mix(conv, S, att, B, N * K, G)
 
     def _dyn1x1_bwd_exact(self, conv, Gt, X, att, B, rps, N, K, G, res):
         """exact-fp32 cross-check of _dyn1x1_bwd: per-sample CUDA-core GEMMs on the materialised mixed kernels"""
@@ -359,8 +276,8 @@ class DyMNEngine(MNEngine):
         dev = Gt.device
         dc = self.dcode
         es = 4 if dc == 0 else 2
-        M, nb, W = B * rps, conv.k, conv.weight
-        Wm = self._mixed_weights(W, att, B, N * K)
+        M = B * rps
+        Wm = self._mixed_weights(conv.weight, att, B, N * K)
         dX = torch.empty(M, K, device=dev, dtype=self.tdtype)
         S = torch.zeros(B, N * K, device=dev, dtype=torch.float32)
         for b in range(B):
@@ -368,9 +285,15 @@ class DyMNEngine(MNEngine):
             L.gemm_simt_fwd(g_b, dc, Wm.data_ptr() + 4 * b * N * K, 1, dX.data_ptr() + b * rps * K * es, dc, rps, K, N,
                             0, 0, 0, 0, 1, 0, 0, 0, (res.data_ptr() + b * rps * K * es) if res is not None else 0, 0, 0, st)
             L.gemm_simt_wgrad(g_b, dc, x_b, dc, S.data_ptr() + 4 * b * N * K, 0, rps, N, K, 0, 0, 0, 0, 1, st)
-        datt = torch.empty(B, nb, device=dev, dtype=torch.float32)
-        L.dyn_wgrad_mix(S.data_ptr(), att.data_ptr(), W.data_ptr(), G[W].data_ptr(), datt.data_ptr(), B, N * K, nb, st)
-        return dX, datt
+        return dX, self._wgrad_mix(conv, S, att, B, N * K, G)
+
+    def _wgrad_mix(self, conv, S, att, B, n, G):
+        """a DynamicConv's kernel-bank gradients (sum_b att[b, k] S_b, into G) and its attention's gradient
+        (<S_b, W_k>, returned [B, k]) from the per-sample weight gradients S [B, n]"""
+        datt = torch.empty(B, conv.k, device=S.device, dtype=torch.float32)
+        lib().dyn_wgrad_mix(S.data_ptr(), att.data_ptr(), conv.weight.data_ptr(), G[conv.weight].data_ptr(), datt.data_ptr(),
+                            B, n, conv.k, _stream())
+        return datt
 
     def _att_bwd(self, conv, datt, att, h_c, dh_c, G, B, H):
         lin = conv.residuals[0]
@@ -380,7 +303,7 @@ class DyMNEngine(MNEngine):
 
     def _block_bwd(self, blk, R, dy, G, B):
         if not blk.dy:
-            return self._ir_block_bwd(blk, R, dy, G, B)
+            return super()._block_bwd(blk, R, dy, G, B)
         L = lib()
         st = _stream()
         dev = dy.device
@@ -406,22 +329,15 @@ class DyMNEngine(MNEngine):
         npc = act_mod.M                                     # DyReLU-B pieces: dcoef [B, C, 2M]
         dcoef = torch.zeros(B, C, 2 * npc, device=dev, dtype=f32)
         du = torch.empty_like(R["z2"])
-        act_args = (dp.data_ptr(), R["z2"].data_ptr(), du.data_ptr(), dc, R["sc2"][0].data_ptr(), R["sc2"][1].data_ptr(),
-                    R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), act_mod.init_v.data_ptr(), R["ca_f"].data_ptr(),
-                    R["ca_t"].data_ptr(), dcaf.data_ptr(), dcat.data_ptr(), dcoef.data_ptr())
-        if npc == 2:
-            L.dy_act_bwd(*act_args, B, Fo, To, C, st)
-        else:
-            L.dy_act_bwd_m(*act_args, npc, B, Fo, To, C, st)
+        L.dy_act_bwd_m(dp.data_ptr(), R["z2"].data_ptr(), du.data_ptr(), dc, *_pair(R["sc2"]), R["theta"].data_ptr(),
+                       act_mod.lambdas.data_ptr(), act_mod.init_v.data_ptr(), R["ca_f"].data_ptr(), R["ca_t"].data_ptr(),
+                       dcaf.data_ptr(), dcat.data_ptr(), dcoef.data_ptr(), npc, B, Fo, To, C, st)
         # DyReLU coefficient net
         coef = act_mod.coef_net[0]
         nco = 2 * npc * C
         dpre = torch.empty(B, nco, device=dev, dtype=f32)
-        if npc == 2:
-            L.dyrelu_coef_bwd(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(), B * nco, st)
-        else:
-            L.dyrelu_coef_bwd_m(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(),
-                                B * nco, npc, st)
+        L.dyrelu_coef_bwd_m(dcoef.data_ptr(), R["theta"].data_ptr(), act_mod.lambdas.data_ptr(), dpre.data_ptr(), B * nco, npc,
+                            st)
         self._wgrad(dpre, h_c, G[coef.weight], G[coef.bias], B, nco, H, g_code=0, a_code=0)
         dh_new = torch.empty_like(dh_c)
         self._gemm(dpre, coef.weight, dh_new, B, H, nco, a_code=0, c_code=0, w_trans=True, res=dh_c)
@@ -442,12 +358,9 @@ class DyMNEngine(MNEngine):
         kk = blk.k * blk.k
         dw_in, dw_sc = R["dw_in"], R["dw_sc"]
         Sdw = torch.zeros(B, C * kk, device=dev, dtype=f32)
-        L.dw_conv_wgrad(dz2.data_ptr(), dw_in.data_ptr(), _ptr(dw_sc[0]) if dw_sc is not None else 0,
-                        _ptr(dw_sc[1]) if dw_sc is not None else 0, blk.act if dw_sc is not None else 0, Sdw.data_ptr(),
-                        C * kk, dc, B, Fi, Ti, C, blk.k, s, st)
-        datt = torch.empty(B, m.depth_conv.k, device=dev, dtype=f32)
-        L.dyn_wgrad_mix(Sdw.data_ptr(), R["att_d"].data_ptr(), m.depth_conv.weight.data_ptr(),
-                        G[m.depth_conv.weight].data_ptr(), datt.data_ptr(), B, C * kk, m.depth_conv.k, st)
+        L.dw_conv_wgrad(dz2.data_ptr(), dw_in.data_ptr(), *_xf(dw_sc, blk.act), Sdw.data_ptr(), C * kk, dc, B, Fi, Ti, C,
+                        blk.k, s, st)
+        datt = self._wgrad_mix(m.depth_conv, Sdw, R["att_d"], B, C * kk, G)
         self._att_bwd(m.depth_conv, datt, R["att_d"], h_c, dh_c, G, B, H)
         da1 = torch.empty_like(dw_in)
         L.dw_conv_dgrad(dz2.data_ptr(), R["wt"].data_ptr(), kk * C, _ptr(dy) if (blk.res and not blk.has_exp) else 0,
