@@ -107,19 +107,32 @@ struct DyEpi {
   long long wt_bstride;  // floats between the weight tables of consecutive samples (0: shared weights)
 };
 
-// DyReLU-B with M linear pieces (dy_block.py:172-188) for one channel.  theta points at the channel's 2M values of
-// sigmoid(coef_net(h_c)), channel-major ([B, C, 2M]); a_m = (2 theta_m - 1) lam_m + init_m is the slope of piece m and
-// b_m = (2 theta_{M+m} - 1) lam_{M+m} + init_{M+m} its offset; out = max_m (a_m x + b_m).  The M = 2 kernels keep their
-// own four-register form; this one serves M = 1, 3, 4 (2M coefficients per channel in registers).
+// DyReLU-B with M linear pieces (dy_block.py:172-188) for one channel, the form every kernel with a DyReLU-B epilogue or
+// backward holds in registers.  theta points at the channel's 2M values of sigmoid(coef_net(h_c)), channel-major
+// ([B, C, 2M]); a_m = (2 theta_m - 1) lam_m + init_m is the slope of piece m and b_m = (2 theta_{M+m} - 1) lam_{M+m} +
+// init_{M+m} its offset; out = max_m (a_m x + b_m).
 template <int M>
 struct DyCoef {
   float a[M], b[M];
-  __device__ __forceinline__ void load(const float* theta, const float* lam, const float* init) {
+  // ldg: read theta through the read-only data cache.  For even M the 2M values are read as 16-byte vectors (theta
+  // 16-byte aligned); lam and init are plain loads.
+  __device__ __forceinline__ void load(const float* theta, const float* lam, const float* init, bool ldg) {
+    float th[2 * M];
+    if constexpr (M % 2 == 0) {
 #pragma unroll
-    for (int m = 0; m < M; ++m) {
-      a[m] = (2.f * __ldg(theta + m) - 1.f) * __ldg(lam + m) + __ldg(init + m);
-      b[m] = (2.f * __ldg(theta + M + m) - 1.f) * __ldg(lam + M + m) + __ldg(init + M + m);
+      for (int q = 0; q < M / 2; ++q) {
+        const float4* p = reinterpret_cast<const float4*>(theta) + q;
+        const float4 t = ldg ? __ldg(p) : *p;
+        th[4 * q] = t.x; th[4 * q + 1] = t.y; th[4 * q + 2] = t.z; th[4 * q + 3] = t.w;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 2 * M; ++j) th[j] = ldg ? __ldg(theta + j) : theta[j];
     }
+#pragma unroll
+    for (int m = 0; m < M; ++m) a[m] = (2.f * th[m] - 1.f) * lam[m] + init[m];
+#pragma unroll
+    for (int m = 0; m < M; ++m) b[m] = (2.f * th[M + m] - 1.f) * lam[M + m] + init[M + m];
   }
   __device__ __forceinline__ void zero() {
 #pragma unroll
@@ -156,6 +169,9 @@ int dw_dgrad2_slide_launch(const void* dz, const float* wt, long long wt_bstride
 // CUDA-core weight gradient for narrow 1x1 convolutions (wgrad_narrow.cu); EAT_ERR_UNSUPPORTED = shape out of range
 int wgrad_narrow_launch(const float* G, const float* A, float* dW, long long M, int N, int K, const float* in_scale,
                         const float* in_shift, int in_act, cudaStream_t st);
+
+// argument checks of the entry points that take per-clip lengths t_valid [B] of a [B, F, T, C] batch (packed.cu)
+int len_check(const char* who, const void* x, int dtype, int B, int F, int T, int C, const int* t_valid);
 
 // C[M, N] = alpha * A[M, K] . W[K, N], fp32, 32 x 32 tiles (gemm_simt.cu)
 int gemm_small_kn_launch(const float* A, const float* W, float* C, int M, int N, int K, float alpha, cudaStream_t st);

@@ -209,9 +209,8 @@ __global__ void __launch_bounds__(kThreads) stem_row_kernel(
 // ((FR-1)*S+K rows x (TT-1)*S+K columns x 32 channels) in shared memory as fp32, applying the producing layer's
 // BatchNorm + activation ONCE per element, then
 // every thread computes a strip of P outputs for one 4-channel vector from shared memory (LDS.128).
-// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue (2: four registers; 1, 3, 4: DyCoef, common.cuh).  The 2 DM
-// coefficients per channel vector stay in registers: DM = 1 at 2 CTAs per SM, DM = 3, 4 at one (no spills; DESIGN.md
-// section 4)
+// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue (DyCoef, common.cuh).  The 2 DM coefficients per channel vector stay
+// in registers: DM = 2 at 3 CTAs per SM, DM = 1 at 2, DM = 3, 4 at one (no spills; DESIGN.md section 4)
 template <typename T, int K, int S, int MODE, int DM = 2>
 __global__ void __launch_bounds__(kThreads, DM == 2 ? 3 : (DM == 1 ? 2 : 1)) dw_tile_kernel(
     const T* __restrict__ in, const float* __restrict__ wt, T* __restrict__ out,
@@ -274,7 +273,6 @@ __global__ void __launch_bounds__(kThreads, DM == 2 ? 3 : (DM == 1 ? 2 : 1)) dw_
   const int c0 = cbase + cvec * 4;
   const bool cvalid = cvec < ccv_valid;
   float osc[4], osh[4], lsum[4] = {0.f, 0.f, 0.f, 0.f}, lsq[4] = {0.f, 0.f, 0.f, 0.f};
-  float da1[4], da2[4], db1[4], db2[4];
   DyCoef<DM> dyc[4];
   if (cvalid) {
     if (kAff && scale != nullptr) {
@@ -282,20 +280,8 @@ __global__ void __launch_bounds__(kThreads, DM == 2 ? 3 : (DM == 1 ? 2 : 1)) dw_
       for (int i = 0; i < 4; ++i) { osc[i] = scale[c0 + i]; osh[i] = shift[c0 + i]; }
     }
     if (kDy && dy.theta != nullptr) {
-      if constexpr (DM == 2) {
-        const float* th = dy.theta + ((size_t)b * C + c0) * 4;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
-          da1[i] = (2.f * t4.x - 1.f) * dy.lam[0] + dy.init[0];
-          da2[i] = (2.f * t4.y - 1.f) * dy.lam[1] + dy.init[1];
-          db1[i] = (2.f * t4.z - 1.f) * dy.lam[2] + dy.init[2];
-          db2[i] = (2.f * t4.w - 1.f) * dy.lam[3] + dy.init[3];
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) dyc[i].load(dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), dy.lam, dy.init);
-      }
+      for (int i = 0; i < 4; ++i) dyc[i].load(dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), dy.lam, dy.init, true);
     }
   }
   for (int tile = grp; tile < tiles_per_chunk; tile += groups) {
@@ -371,13 +357,8 @@ __global__ void __launch_bounds__(kThreads, DM == 2 ? 3 : (DM == 1 ? 2 : 1)) dw_
             }
           }
           if (kDy && dy.theta != nullptr) {
-            if constexpr (DM == 2) {
 #pragma unroll
-              for (int i = 0; i < 4; ++i) o[i] = fmaxf(fmaf(o[i], da1[i], db1[i]), fmaf(o[i], da2[i], db2[i]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) o[i] = dyc[i].apply(o[i]);
-            }
+            for (int i = 0; i < 4; ++i) o[i] = dyc[i].apply(o[i]);
           }
           if (kDy && dy.ca_f != nullptr) {
             const float4 f4 = __ldg(reinterpret_cast<const float4*>(dy.ca_f + ((size_t)b * Fo + fo) * C + c0));

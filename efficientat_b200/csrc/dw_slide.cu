@@ -99,8 +99,7 @@ struct SlideArgs {
 // D = 2: dilation 2 at stride 1.  Such a layer is four independent undilated K x K convolutions, one on each (row parity,
 // column parity) sub-grid of the image, so a unit walks rows and columns of one parity: the same walk with row and column
 // steps of two pixels.  Each sample has D * D times the units of one sub-grid; D = 1 is the undilated kernel.
-// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue.  DM = 2 is the four-register form; 1, 3 and 4 hold 2 DM coefficients
-// per channel in registers (DyCoef, common.cuh).
+// DM: DyReLU-B pieces of the MODE 1 DyMN epilogue, 2 DM coefficients per channel in registers (DyCoef, common.cuh).
 template <typename T, int K, int S, int P, int MODE, int XACT, int MINB, bool RING, int D = 1, int DM = 2>
 __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) {
   static_assert(D == 1 || (D == 2 && S == 1), "dilation 2 is stride 1 only");
@@ -162,23 +161,10 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
 #pragma unroll
       for (int i = 0; i < V; ++i) { osc[i] = __ldg(a.scale + c0 + i); osh[i] = __ldg(a.shift + c0 + i); }
     }
-    float da1[V], da2[V], db1[V], db2[V];
     DyCoef<DM> dyc[V];
     if (kDy && a.dy.theta != nullptr) {
-      if constexpr (DM == 2) {
-        const float* th = a.dy.theta + ((size_t)b * C + c0) * 4;
 #pragma unroll
-        for (int i = 0; i < V; ++i) {
-          const float4 t4 = __ldg(reinterpret_cast<const float4*>(th) + i);
-          da1[i] = (2.f * t4.x - 1.f) * a.dy.lam[0] + a.dy.init[0];
-          da2[i] = (2.f * t4.y - 1.f) * a.dy.lam[1] + a.dy.init[1];
-          db1[i] = (2.f * t4.z - 1.f) * a.dy.lam[2] + a.dy.init[2];
-          db2[i] = (2.f * t4.w - 1.f) * a.dy.lam[3] + a.dy.init[3];
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < V; ++i) dyc[i].load(a.dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), a.dy.lam, a.dy.init);
-      }
+      for (int i = 0; i < V; ++i) dyc[i].load(a.dy.theta + ((size_t)b * C + c0 + i) * (2 * DM), a.dy.lam, a.dy.init, true);
     }
     int bb = b;                                  // sample of the current unit
     const T* inb = nullptr;
@@ -222,13 +208,8 @@ __global__ void __launch_bounds__(kST, MINB) dw_slide_kernel(const SlideArgs a) 
             ++nsum;
           }
           if (kDy && a.dy.theta != nullptr) {
-            if constexpr (DM == 2) {
 #pragma unroll
-              for (int i = 0; i < V; ++i) o[p][i] = fmaxf(fmaf(o[p][i], da1[i], db1[i]), fmaf(o[p][i], da2[i], db2[i]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < V; ++i) o[p][i] = dyc[i].apply(o[p][i]);
-            }
+            for (int i = 0; i < V; ++i) o[p][i] = dyc[i].apply(o[p][i]);
           }
           if (kDy && a.dy.ca_f != nullptr) {
             const float* cf = a.dy.ca_f + ((size_t)bb * Fo + fo) * C + c0;

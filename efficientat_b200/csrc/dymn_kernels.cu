@@ -2,18 +2,21 @@
 //   ContextGen pooling (:236-237), sequence average pooling (:227-233,249), DynamicConv attention
 //   softmax(Linear(h_c)/T) (:104-107) and the per-sample depthwise weight mix (:111-117).
 #include <cstdio>
+#include <type_traits>
 
 #include "common.cuh"
 
 namespace {
 
-// out[b, pos, c]: pos < F -> mean over t of x[b, pos, :, c];  pos >= F -> mean over f of x[b, :, pos-F, c]
-template <typename T>
+// out[b, pos, c]: pos < F -> mean over t < T_b of x[b, pos, t, c];  pos = F + t -> mean over f of x[b, :, t, c] for
+// t < T_b, 0 beyond.  T_b = t_valid[b] with LEN (clips of different lengths, see packed.cu), T without.
+template <typename T, bool LEN = false>
 __global__ void __launch_bounds__(256) ctx_pool_kernel(const T* __restrict__ x, float* __restrict__ out, int F, int Tn,
-                                                       int C) {
+                                                       int C, const int* __restrict__ t_valid) {
   constexpr int V = Vec<T>::N;
   const int cv = C / V;
   const int b = blockIdx.y;
+  const int tb = LEN ? t_valid[b] : Tn;
   const int items = (F + Tn) * cv;
   const T* xb = x + (size_t)b * F * Tn * C;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < items; i += gridDim.x * blockDim.x) {
@@ -24,16 +27,16 @@ __global__ void __launch_bounds__(256) ctx_pool_kernel(const T* __restrict__ x, 
     for (int k = 0; k < V; ++k) acc[k] = 0.f;
     if (pos < F) {
       const T* p = xb + (size_t)pos * Tn * C + c0;
-      for (int t = 0; t < Tn; ++t) {
+      for (int t = 0; t < tb; ++t) {
         float v[V];
         Vec<T>::load(p + (size_t)t * C, v);
 #pragma unroll
         for (int k = 0; k < V; ++k) acc[k] += v[k];
       }
-      const float inv = 1.f / Tn;
+      const float inv = 1.f / tb;
 #pragma unroll
       for (int k = 0; k < V; ++k) acc[k] *= inv;
-    } else {
+    } else if (!LEN || pos - F < tb) {
       const T* p = xb + (size_t)(pos - F) * C + c0;
       for (int f = 0; f < F; ++f) {
         float v[V];
@@ -133,13 +136,15 @@ template <> struct V4<__nv_bfloat16> {
 
 struct DyActCtx {
   const float* scale; const float* shift;   // BatchNorm affine of the depthwise output [C]
-  const float* theta;                       // [B, C, 4] sigmoid(coef_net(h_c))
-  const float* lam; const float* init;      // DyReLU buffers [4]
+  const float* theta;                       // [B, C, 2M] sigmoid(coef_net(h_c)), M = DyReLU-B pieces
+  const float* lam; const float* init;      // DyReLU buffers [2M]
   const float* ca_f; const float* ca_t;     // [B, Fo, C], [B, To, C]
 };
 
-// p = max(u a1 + b1, u a2 + b2) * ca_f * ca_t,  u = z * scale + shift        (dy_block.py:400-402)
-template <typename T>
+// DyReLU-B with DM linear pieces (dyrelu_k), theta [B, C, 2 DM] channel-major:
+// p = max_m (u a_m + b_m) * ca_f * ca_t,  u = z * scale + shift     (dy_block.py:179-188, 400-402); DM = 1 is the affine
+// map u a_0 + b_0
+template <typename T, int DM = 2>
 __global__ void __launch_bounds__(256) dy_act_fwd_kernel(const T* __restrict__ z, T* __restrict__ out, DyActCtx c, int Fo,
                                                          int To, int C) {
   const int b = blockIdx.y;
@@ -157,150 +162,25 @@ __global__ void __launch_bounds__(256) dy_act_fwd_kernel(const T* __restrict__ z
     const float q[4] = {f4.x * t4.x, f4.y * t4.y, f4.z * t4.z, f4.w * t4.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float4 th = *reinterpret_cast<const float4*>(c.theta + ((size_t)b * C + c0 + k) * 4);
-      const float a1 = (2.f * th.x - 1.f) * c.lam[0] + c.init[0], a2 = (2.f * th.y - 1.f) * c.lam[1] + c.init[1];
-      const float b1 = (2.f * th.z - 1.f) * c.lam[2] + c.init[2], b2 = (2.f * th.w - 1.f) * c.lam[3] + c.init[3];
-      const float u = fmaf(v[k], c.scale[c0 + k], c.shift[c0 + k]);
-      v[k] = fmaxf(fmaf(u, a1, b1), fmaf(u, a2, b2)) * q[k];
-    }
-    V4<T>::store(out + off, v);
-  }
-}
-
-// Backward of the above.  CTA = (32 output columns x 32 channels) of one sample, each thread walks all Fo rows of
-// its (to, 4-channel) column: d(ca_t) is complete in registers, d(ca_f) and the DyReLU coefficient gradients are
-// reduced in shared memory and added to global memory once per CTA.
-template <typename T>
-__global__ void __launch_bounds__(256) dy_act_bwd_kernel(const T* __restrict__ dp, const T* __restrict__ z, DyActCtx c,
-                                                         T* __restrict__ du, float* __restrict__ dcaf,
-                                                         float* __restrict__ dcat, float* __restrict__ dcoef, int Fo,
-                                                         int To, int C) {
-  extern __shared__ float smem[];
-  float* s_caf = smem;              // [Fo][32]
-  float* s_coef = smem + Fo * 32;   // [32][4]
-  const int b = blockIdx.y;
-  const int chunks = ceil_div(C, 32);
-  const int chunk = blockIdx.x % chunks, tblk = blockIdx.x / chunks;
-  const int cvec = threadIdx.x & 7, tslot = threadIdx.x >> 3;
-  const int c0 = chunk * 32 + cvec * 4, to = tblk * 32 + tslot;
-  for (int i = threadIdx.x; i < Fo * 32 + 128; i += 256) smem[i] = 0.f;
-  __syncthreads();
-  const bool live = c0 < C && to < To;
-  float a1[4], a2[4], b1[4], b2[4], sc[4], sh[4], ct[4];
-  float g_ct[4] = {0.f, 0.f, 0.f, 0.f}, g_a1[4] = {0.f, 0.f, 0.f, 0.f}, g_a2[4] = {0.f, 0.f, 0.f, 0.f};
-  float g_b1[4] = {0.f, 0.f, 0.f, 0.f}, g_b2[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) { a1[k] = a2[k] = b1[k] = b2[k] = sc[k] = sh[k] = ct[k] = 0.f; }
-  if (live) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float4 th = *reinterpret_cast<const float4*>(c.theta + ((size_t)b * C + c0 + k) * 4);
-      a1[k] = (2.f * th.x - 1.f) * c.lam[0] + c.init[0]; a2[k] = (2.f * th.y - 1.f) * c.lam[1] + c.init[1];
-      b1[k] = (2.f * th.z - 1.f) * c.lam[2] + c.init[2]; b2[k] = (2.f * th.w - 1.f) * c.lam[3] + c.init[3];
-      sc[k] = c.scale[c0 + k]; sh[k] = c.shift[c0 + k];
-    }
-    const float4 t4 = *reinterpret_cast<const float4*>(c.ca_t + ((size_t)b * To + to) * C + c0);
-    ct[0] = t4.x; ct[1] = t4.y; ct[2] = t4.z; ct[3] = t4.w;
-  }
-  // every thread walks the rows (the d(ca_f) partial sums of the four output columns a warp holds for one channel vector
-  // are combined with shuffles before they reach shared memory: one atomic per channel and warp instead of four
-  // conflicting ones -- shared fp32 atomics are compare-and-swap loops)
-  for (int fo = 0; fo < Fo; ++fo) {
-    float dcf[4] = {0.f, 0.f, 0.f, 0.f};
-    if (live) {
-      const size_t off = (((size_t)b * Fo + fo) * To + to) * C + c0;
-      float g[4], zv[4], o[4];
-      V4<T>::load(dp + off, g);
-      V4<T>::load(z + off, zv);
-      const float4 f4 = *reinterpret_cast<const float4*>(c.ca_f + ((size_t)b * Fo + fo) * C + c0);
-      const float cf[4] = {f4.x, f4.y, f4.z, f4.w};
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const float u = fmaf(zv[k], sc[k], sh[k]);
-        const float l1 = fmaf(u, a1[k], b1[k]), l2 = fmaf(u, a2[k], b2[k]);
-        const bool sel = l1 >= l2;
-        const float r = sel ? l1 : l2;
-        const float dr = g[k] * cf[k] * ct[k];
-        dcf[k] = g[k] * r * ct[k];
-        g_ct[k] = fmaf(g[k] * r, cf[k], g_ct[k]);
-        o[k] = dr * (sel ? a1[k] : a2[k]);
-        if (sel) { g_a1[k] = fmaf(dr, u, g_a1[k]); g_b1[k] += dr; } else { g_a2[k] = fmaf(dr, u, g_a2[k]); g_b2[k] += dr; }
-      }
-      V4<T>::store(du + off, o);
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      dcf[k] += __shfl_xor_sync(0xffffffffu, dcf[k], 8);
-      dcf[k] += __shfl_xor_sync(0xffffffffu, dcf[k], 16);
-    }
-    if ((threadIdx.x & 31) < 8) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) atomicAdd(&s_caf[fo * 32 + cvec * 4 + k], dcf[k]);
-    }
-  }
-  // DyReLU coefficient gradients: same shuffle combine, then one atomic per coefficient and warp
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    float v[4] = {g_a1[k], g_a2[k], g_b1[k], g_b2[k]};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      v[j] += __shfl_xor_sync(0xffffffffu, v[j], 8);
-      v[j] += __shfl_xor_sync(0xffffffffu, v[j], 16);
-      if ((threadIdx.x & 31) < 8) atomicAdd(&s_coef[(cvec * 4 + k) * 4 + j], v[j]);
-    }
-  }
-  if (live) {
-    float* dct = dcat + ((size_t)b * To + to) * C + c0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) dct[k] = g_ct[k];
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < Fo * 32; i += 256) {
-    const int fo = i / 32, cc = chunk * 32 + (i & 31);
-    if (cc < C) atomicAdd(dcaf + ((size_t)b * Fo + fo) * C + cc, s_caf[i]);
-  }
-  if (threadIdx.x < 128) {
-    const int cc = chunk * 32 + (threadIdx.x >> 2);
-    if (cc < C) atomicAdd(dcoef + ((size_t)b * C + cc) * 4 + (threadIdx.x & 3), s_coef[threadIdx.x]);
-  }
-}
-
-// ---- DyReLU-B with DM = 1, 3 or 4 linear pieces (dyrelu_k; theta [B, C, 2 DM] channel-major).  The kernels above are the
-// DM = 2 instances.  p = max_m (u a_m + b_m) * ca_f * ca_t (dy_block.py:179-188); DM = 1 is the affine map u a_0 + b_0.
-template <typename T, int DM>
-__global__ void __launch_bounds__(256) dy_act_fwd_m_kernel(const T* __restrict__ z, T* __restrict__ out, DyActCtx c,
-                                                           int Fo, int To, int C) {
-  const int b = blockIdx.y;
-  const int cv = C / 4;
-  const long long nvec = (long long)Fo * To * cv;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
-    const int c0 = (int)(i % cv) * 4;
-    const long long pix = i / cv;
-    const int to = (int)(pix % To), fo = (int)(pix / To);
-    const size_t off = ((size_t)b * Fo * To + pix) * C + c0;
-    float v[4];
-    V4<T>::load(z + off, v);
-    const float4 f4 = *reinterpret_cast<const float4*>(c.ca_f + ((size_t)b * Fo + fo) * C + c0);
-    const float4 t4 = *reinterpret_cast<const float4*>(c.ca_t + ((size_t)b * To + to) * C + c0);
-    const float q[4] = {f4.x * t4.x, f4.y * t4.y, f4.z * t4.z, f4.w * t4.w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
       DyCoef<DM> co;
-      co.load(c.theta + ((size_t)b * C + c0 + k) * (2 * DM), c.lam, c.init);
+      co.load(c.theta + ((size_t)b * C + c0 + k) * (2 * DM), c.lam, c.init, false);
       v[k] = co.apply(fmaf(v[k], c.scale[c0 + k], c.shift[c0 + k])) * q[k];
     }
     V4<T>::store(out + off, v);
   }
 }
 
-// Backward of the above, laid out as dy_act_bwd_kernel (s_coef holds 2 DM sums per channel).  Each pixel's gradient goes
-// to the piece that attains the max; on a tie, to the lowest piece index (the M = 2 kernel's `l1 >= l2` rule; the
-// reference's torch.max(dim=-1) also returns one index).
-template <typename T, int DM>
-__global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__ dp, const T* __restrict__ z, DyActCtx c,
-                                                           T* __restrict__ du, float* __restrict__ dcaf,
-                                                           float* __restrict__ dcat, float* __restrict__ dcoef, int Fo,
-                                                           int To, int C) {
+// Backward of the above.  CTA = (32 output columns x 32 channels) of one sample, each thread walks all Fo rows of
+// its (to, 4-channel) column: d(ca_t) is complete in registers, d(ca_f) and the DyReLU coefficient gradients (2 DM sums
+// per channel) are reduced in shared memory and added to global memory once per CTA.  Each pixel's gradient goes to the
+// one piece that attains the max (the reference's torch.max(dim=-1) also returns one index): the walk moves on to piece m
+// when !(r >= l_m), r the max so far, so a tie stays with the lowest index and a NaN on either side moves on.  At DM = 2
+// that is piece 0 iff l_0 >= l_1.
+template <typename T, int DM = 2>
+__global__ void __launch_bounds__(256) dy_act_bwd_kernel(const T* __restrict__ dp, const T* __restrict__ z, DyActCtx c,
+                                                         T* __restrict__ du, float* __restrict__ dcaf,
+                                                         float* __restrict__ dcat, float* __restrict__ dcoef, int Fo,
+                                                         int To, int C) {
   constexpr int NC = 2 * DM;
   extern __shared__ float smem[];
   float* s_caf = smem;              // [Fo][32]
@@ -325,12 +205,15 @@ __global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__
   if (live) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      co[k].load(c.theta + ((size_t)b * C + c0 + k) * NC, c.lam, c.init);
+      co[k].load(c.theta + ((size_t)b * C + c0 + k) * NC, c.lam, c.init, false);
       sc[k] = c.scale[c0 + k]; sh[k] = c.shift[c0 + k];
     }
     const float4 t4 = *reinterpret_cast<const float4*>(c.ca_t + ((size_t)b * To + to) * C + c0);
     ct[0] = t4.x; ct[1] = t4.y; ct[2] = t4.z; ct[3] = t4.w;
   }
+  // every thread walks the rows (the d(ca_f) partial sums of the four output columns a warp holds for one channel vector
+  // are combined with shuffles before they reach shared memory: one atomic per channel and warp instead of four
+  // conflicting ones -- shared fp32 atomics are compare-and-swap loops)
   for (int fo = 0; fo < Fo; ++fo) {
     float dcf[4] = {0.f, 0.f, 0.f, 0.f};
     if (live) {
@@ -348,7 +231,7 @@ __global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__
 #pragma unroll
         for (int m = 1; m < DM; ++m) {
           const float l = fmaf(u, co[k].a[m], co[k].b[m]);
-          if (l > r) { r = l; slope = co[k].a[m]; arg = m; }
+          if (!(r >= l)) { r = l; slope = co[k].a[m]; arg = m; }
         }
         const float dr = g[k] * cf[k] * ct[k];
         dcf[k] = g[k] * r * ct[k];
@@ -370,6 +253,7 @@ __global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__
       for (int k = 0; k < 4; ++k) atomicAdd(&s_caf[fo * 32 + cvec * 4 + k], dcf[k]);
     }
   }
+  // DyReLU coefficient gradients: same shuffle combine, then one atomic per coefficient and warp
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
 #pragma unroll
@@ -396,22 +280,14 @@ __global__ void __launch_bounds__(256) dy_act_bwd_m_kernel(const T* __restrict__
   }
 }
 
-// dpre[i] = dcoef[i] * lam[i % 2DM] * 2 s (1 - s), s = theta[i]: dyrelu_coef_bwd_kernel for DM pieces
-template <int DM>
-__global__ void dyrelu_coef_bwd_m_kernel(const float* __restrict__ dcoef, const float* __restrict__ theta,
-                                         const float* __restrict__ lam, float* __restrict__ dpre, long long n) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float s = theta[i];
-    dpre[i] = dcoef[i] * lam[i % (2 * DM)] * 2.f * s * (1.f - s);
-  }
-}
-
-// dpre[b,c,j] = dcoef[b,c,j] * lam[j] * 2 * s (1 - s),  s = theta[b,c,j]      (DyReLU coefficient net, dy_block.py:157-160,179)
+// dpre[b,c,j] = dcoef[b,c,j] * lam[j] * 2 * s (1 - s),  s = theta[b,c,j], j < 2 DM      (DyReLU coefficient net,
+// dy_block.py:157-160,179)
+template <int DM = 2>
 __global__ void dyrelu_coef_bwd_kernel(const float* __restrict__ dcoef, const float* __restrict__ theta,
                                        const float* __restrict__ lam, float* __restrict__ dpre, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float s = theta[i];
-    dpre[i] = dcoef[i] * lam[i & 3] * 2.f * s * (1.f - s);
+    dpre[i] = dcoef[i] * lam[i % (2 * DM)] * 2.f * s * (1.f - s);
   }
 }
 // out = g * s * (1 - s)
@@ -558,6 +434,56 @@ __global__ void zero_kernel(float* __restrict__ p, int n) {
   if (i < n) p[i] = 0.f;
 }
 
+inline int ew_grid(long long n) { long long g = ceil_div_ll(n, 256); return (int)(g > kNumSMs * 16 ? kNumSMs * 16 : (g < 1 ? 1 : g)); }
+
+// f(std::integral_constant<int, M>{}) for M = pieces, which the caller has checked to be 1..4
+template <typename Fn>
+void with_pieces(int pieces, Fn&& f) {
+  switch (pieces) {
+    case 1: f(std::integral_constant<int, 1>{}); break;
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 3: f(std::integral_constant<int, 3>{}); break;
+    default: f(std::integral_constant<int, 4>{}); break;
+  }
+}
+
+// launchers of the DyReLU-B kernels, shared by the entry points with 2 and with `pieces` linear pieces; B >= 1
+int dy_act_fwd_launch(const void* z, void* out, int dtype, DyActCtx c, int pieces, int B, int Fo, int To, int C,
+                      cudaStream_t st) {
+  dim3 grid(max(1, min(kNumSMs * 8 / max(B, 1) + 1, (int)ceil_div_ll((long long)Fo * To * (C / 4), 256))), B);
+  with_pieces(pieces, [&](auto dm) {
+    constexpr int DM = decltype(dm)::value;
+    if (dtype == EAT_BF16) dy_act_fwd_kernel<__nv_bfloat16, DM><<<grid, 256, 0, st>>>((const __nv_bfloat16*)z, (__nv_bfloat16*)out, c, Fo, To, C);
+    else dy_act_fwd_kernel<float, DM><<<grid, 256, 0, st>>>((const float*)z, (float*)out, c, Fo, To, C);
+  });
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int dy_act_bwd_launch(const void* dp, const void* z, void* du, int dtype, DyActCtx c, float* dcaf, float* dcat,
+                      float* dcoef, int pieces, int B, int Fo, int To, int C, cudaStream_t st) {
+  dim3 grid(ceil_div(C, 32) * ceil_div(To, 32), B);
+  const size_t smem = ((size_t)Fo * 32 + 32 * 2 * pieces) * sizeof(float);
+  with_pieces(pieces, [&](auto dm) {
+    constexpr int DM = decltype(dm)::value;
+    if (dtype == EAT_BF16)
+      dy_act_bwd_kernel<__nv_bfloat16, DM><<<grid, 256, smem, st>>>((const __nv_bfloat16*)dp, (const __nv_bfloat16*)z, c, (__nv_bfloat16*)du, dcaf, dcat, dcoef, Fo, To, C);
+    else
+      dy_act_bwd_kernel<float, DM><<<grid, 256, smem, st>>>((const float*)dp, (const float*)z, c, (float*)du, dcaf, dcat, dcoef, Fo, To, C);
+  });
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int dyrelu_coef_bwd_launch(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n,
+                           int pieces, cudaStream_t st) {
+  with_pieces(pieces, [&](auto dm) {
+    dyrelu_coef_bwd_kernel<decltype(dm)::value><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
+  });
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -567,8 +493,22 @@ int eat_ctx_pool(const void* x, int dtype, float* out, int B, int F, int T, int 
   const int V = dtype == EAT_BF16 ? 8 : 4;
   if (C % V != 0) { eat_set_error("ctx_pool: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
   dim3 grid(ceil_div((F + T) * (C / V), 256), B);
-  if (dtype == EAT_BF16) ctx_pool_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, out, F, T, C);
-  else ctx_pool_kernel<float><<<grid, 256, 0, st>>>((const float*)x, out, F, T, C);
+  if (dtype == EAT_BF16) ctx_pool_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, out, F, T, C, nullptr);
+  else ctx_pool_kernel<float><<<grid, 256, 0, st>>>((const float*)x, out, F, T, C, nullptr);
+  EAT_CHECK_LAUNCH();
+  return EAT_OK;
+}
+
+int eat_ctx_pool_len(const void* x, int dtype, float* out, int B, int F, int T, int C, const int* t_valid,
+                     cudaStream_t st) {
+  if (int rc = len_check("ctx_pool_len", x, dtype, B, F, T, C, t_valid)) return rc;
+  const int V = dtype == EAT_BF16 ? 8 : 4;
+  if (C % V != 0) { eat_set_error("ctx_pool_len: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
+  if (B == 0) return EAT_OK;
+  if (out == nullptr) { eat_set_error("ctx_pool_len: out is required"); return EAT_ERR_ARG; }
+  const dim3 grid(ceil_div((F + T) * (C / V), 256), B);
+  if (dtype == EAT_BF16) ctx_pool_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, out, F, T, C, t_valid);
+  else ctx_pool_kernel<float, true><<<grid, 256, 0, st>>>((const float*)x, out, F, T, C, t_valid);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }
@@ -613,19 +553,12 @@ int eat_dyconv_mix_dw(const float* w, const float* att, float* wt, int B, int C,
 }
 
 
-static inline int ew_grid(long long n) { long long g = ceil_div_ll(n, 256); return (int)(g > kNumSMs * 16 ? kNumSMs * 16 : (g < 1 ? 1 : g)); }
-
 int eat_dy_act_fwd(const void* z, void* out, int dtype, const float* scale, const float* shift, const float* theta,
                    const float* lam, const float* init, const float* ca_f, const float* ca_t, int B, int Fo, int To,
                    int C, cudaStream_t st) {
   if (B == 0) return EAT_OK;
   if (C % 4 != 0) { eat_set_error("dy_act: channels must be a multiple of 4"); return EAT_ERR_ARG; }
-  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
-  dim3 grid(max(1, min(kNumSMs * 8 / max(B, 1) + 1, (int)ceil_div_ll((long long)Fo * To * (C / 4), 256))), B);
-  if (dtype == EAT_BF16) dy_act_fwd_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)z, (__nv_bfloat16*)out, c, Fo, To, C);
-  else dy_act_fwd_kernel<float><<<grid, 256, 0, st>>>((const float*)z, (float*)out, c, Fo, To, C);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dy_act_fwd_launch(z, out, dtype, DyActCtx{scale, shift, theta, lam, init, ca_f, ca_t}, 2, B, Fo, To, C, st);
 }
 
 int eat_dy_act_bwd(const void* dp, const void* z, void* du, int dtype, const float* scale, const float* shift,
@@ -633,22 +566,13 @@ int eat_dy_act_bwd(const void* dp, const void* z, void* du, int dtype, const flo
                    float* dcaf, float* dcat, float* dcoef, int B, int Fo, int To, int C, cudaStream_t st) {
   if (B == 0) return EAT_OK;
   if (C % 4 != 0) { eat_set_error("dy_act: channels must be a multiple of 4"); return EAT_ERR_ARG; }
-  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
-  dim3 grid(ceil_div(C, 32) * ceil_div(To, 32), B);
-  size_t smem = ((size_t)Fo * 32 + 128) * sizeof(float);
-  if (dtype == EAT_BF16)
-    dy_act_bwd_kernel<__nv_bfloat16><<<grid, 256, smem, st>>>((const __nv_bfloat16*)dp, (const __nv_bfloat16*)z, c, (__nv_bfloat16*)du, dcaf, dcat, dcoef, Fo, To, C);
-  else
-    dy_act_bwd_kernel<float><<<grid, 256, smem, st>>>((const float*)dp, (const float*)z, c, (float*)du, dcaf, dcat, dcoef, Fo, To, C);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dy_act_bwd_launch(dp, z, du, dtype, DyActCtx{scale, shift, theta, lam, init, ca_f, ca_t}, dcaf, dcat, dcoef, 2,
+                           B, Fo, To, C, st);
 }
 
 int eat_dyrelu_coef_bwd(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n, cudaStream_t st) {
   if (n == 0) return EAT_OK;
-  dyrelu_coef_bwd_kernel<<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dyrelu_coef_bwd_launch(dcoef, theta, lam, dpre, n, 2, st);
 }
 
 // argument checks of the DyReLU-B entry points with M pieces, before any launch
@@ -672,20 +596,7 @@ int eat_dy_act_fwd_m(const void* z, void* out, int dtype, const float* scale, co
   const bool null_ptr = !z || !out || !scale || !shift || !theta || !lam || !init || !ca_f || !ca_t;
   if (int rc = dym_check("dy_act_fwd_m", dtype, B, Fo, To, C, pieces, null_ptr)) return rc;
   if (B == 0) return EAT_OK;
-  if (pieces == 2) return eat_dy_act_fwd(z, out, dtype, scale, shift, theta, lam, init, ca_f, ca_t, B, Fo, To, C, st);
-  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
-  dim3 grid(max(1, min(kNumSMs * 8 / max(B, 1) + 1, (int)ceil_div_ll((long long)Fo * To * (C / 4), 256))), B);
-#define EAT_DYF(DM)                                                                                                      \
-  do {                                                                                                                   \
-    if (dtype == EAT_BF16) dy_act_fwd_m_kernel<__nv_bfloat16, DM><<<grid, 256, 0, st>>>((const __nv_bfloat16*)z, (__nv_bfloat16*)out, c, Fo, To, C); \
-    else dy_act_fwd_m_kernel<float, DM><<<grid, 256, 0, st>>>((const float*)z, (float*)out, c, Fo, To, C);            \
-  } while (0)
-  if (pieces == 1) EAT_DYF(1);
-  else if (pieces == 3) EAT_DYF(3);
-  else EAT_DYF(4);
-#undef EAT_DYF
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dy_act_fwd_launch(z, out, dtype, DyActCtx{scale, shift, theta, lam, init, ca_f, ca_t}, pieces, B, Fo, To, C, st);
 }
 
 int eat_dy_act_bwd_m(const void* dp, const void* z, void* du, int dtype, const float* scale, const float* shift,
@@ -695,24 +606,8 @@ int eat_dy_act_bwd_m(const void* dp, const void* z, void* du, int dtype, const f
                         !dcat || !dcoef;
   if (int rc = dym_check("dy_act_bwd_m", dtype, B, Fo, To, C, pieces, null_ptr)) return rc;
   if (B == 0) return EAT_OK;
-  if (pieces == 2)
-    return eat_dy_act_bwd(dp, z, du, dtype, scale, shift, theta, lam, init, ca_f, ca_t, dcaf, dcat, dcoef, B, Fo, To, C, st);
-  DyActCtx c{scale, shift, theta, lam, init, ca_f, ca_t};
-  dim3 grid(ceil_div(C, 32) * ceil_div(To, 32), B);
-  const size_t smem = ((size_t)Fo * 32 + 32 * 2 * pieces) * sizeof(float);
-#define EAT_DYB(DM)                                                                                                      \
-  do {                                                                                                                   \
-    if (dtype == EAT_BF16)                                                                                               \
-      dy_act_bwd_m_kernel<__nv_bfloat16, DM><<<grid, 256, smem, st>>>((const __nv_bfloat16*)dp, (const __nv_bfloat16*)z, c, (__nv_bfloat16*)du, dcaf, dcat, dcoef, Fo, To, C); \
-    else                                                                                                                 \
-      dy_act_bwd_m_kernel<float, DM><<<grid, 256, smem, st>>>((const float*)dp, (const float*)z, c, (float*)du, dcaf, dcat, dcoef, Fo, To, C); \
-  } while (0)
-  if (pieces == 1) EAT_DYB(1);
-  else if (pieces == 3) EAT_DYB(3);
-  else EAT_DYB(4);
-#undef EAT_DYB
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dy_act_bwd_launch(dp, z, du, dtype, DyActCtx{scale, shift, theta, lam, init, ca_f, ca_t}, dcaf, dcat, dcoef,
+                           pieces, B, Fo, To, C, st);
 }
 
 int eat_dyrelu_coef_bwd_m(const float* dcoef, const float* theta, const float* lam, float* dpre, long long n, int pieces,
@@ -730,12 +625,7 @@ int eat_dyrelu_coef_bwd_m(const float* dcoef, const float* theta, const float* l
   }
   if (!dcoef || !theta || !lam || !dpre) { eat_set_error("dyrelu_coef_bwd_m: every tensor pointer is required"); return EAT_ERR_ARG; }
   if (n == 0) return EAT_OK;
-  if (pieces == 2) return eat_dyrelu_coef_bwd(dcoef, theta, lam, dpre, n, st);
-  if (pieces == 1) dyrelu_coef_bwd_m_kernel<1><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
-  else if (pieces == 3) dyrelu_coef_bwd_m_kernel<3><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
-  else dyrelu_coef_bwd_m_kernel<4><<<ew_grid(n), 256, 0, st>>>(dcoef, theta, lam, dpre, n);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
+  return dyrelu_coef_bwd_launch(dcoef, theta, lam, dpre, n, pieces, st);
 }
 
 int eat_sigmoid_bwd(const float* g, const float* s, float* out, long long n, cudaStream_t st) {

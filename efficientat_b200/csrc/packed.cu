@@ -4,7 +4,8 @@
 //   eat_time_pad_zero  writes 0 into the padding, so that a convolution's taps past a clip's end read what its own
 //                      zero padding would supply;
 //   eat_mean_len       the mean over the valid region only (squeeze-excitation, global average pool, ContextGen's h_c);
-//   eat_ctx_pool_len   ContextGen's pair of means (dy_block.py:236-240) with the mean over time taken over t < t_valid.
+//   eat_ctx_pool_len   ContextGen's pair of means (dy_block.py:236-240) with the mean over time taken over t < t_valid
+//                      (dymn_kernels.cu, next to eat_ctx_pool).
 // None of them uses atomics: the sums run in a fixed order, so the results do not depend on the padding's content.
 #include <cstdio>
 
@@ -52,50 +53,7 @@ __global__ void __launch_bounds__(kMeanLanes * kMeanRows) mean_len_kernel(const 
   }
 }
 
-// rows f < F: mean over t < t_valid[b]; rows F + t: mean over f for t < t_valid[b], 0 beyond
-template <typename T>
-__global__ void __launch_bounds__(256) ctx_pool_len_kernel(const T* __restrict__ x, float* __restrict__ out, int F, int Tn,
-                                                           int C, const int* __restrict__ t_valid) {
-  constexpr int V = Vec<T>::N;
-  const int cv = C / V;
-  const int b = blockIdx.y;
-  const int tb = t_valid[b];
-  const int items = (F + Tn) * cv;
-  const T* xb = x + (size_t)b * F * Tn * C;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < items; i += gridDim.x * blockDim.x) {
-    const int cvi = i % cv, pos = i / cv;
-    const int c0 = cvi * V;
-    float acc[V];
-#pragma unroll
-    for (int k = 0; k < V; ++k) acc[k] = 0.f;
-    if (pos < F) {
-      const T* p = xb + (size_t)pos * Tn * C + c0;
-      for (int t = 0; t < tb; ++t) {
-        float v[V];
-        Vec<T>::load(p + (size_t)t * C, v);
-#pragma unroll
-        for (int k = 0; k < V; ++k) acc[k] += v[k];
-      }
-      const float inv = 1.f / tb;
-#pragma unroll
-      for (int k = 0; k < V; ++k) acc[k] *= inv;
-    } else if (pos - F < tb) {
-      const T* p = xb + (size_t)(pos - F) * C + c0;
-      for (int f = 0; f < F; ++f) {
-        float v[V];
-        Vec<T>::load(p + (size_t)f * Tn * C, v);
-#pragma unroll
-        for (int k = 0; k < V; ++k) acc[k] += v[k];
-      }
-      const float inv = 1.f / F;
-#pragma unroll
-      for (int k = 0; k < V; ++k) acc[k] *= inv;
-    }
-    float* o = out + ((size_t)b * (F + Tn) + pos) * C + c0;
-#pragma unroll
-    for (int k = 0; k < V; ++k) o[k] = acc[k];
-  }
-}
+}  // namespace
 
 int len_check(const char* who, const void* x, int dtype, int B, int F, int T, int C, const int* t_valid) {
   static char msg[200];
@@ -111,8 +69,6 @@ int len_check(const char* who, const void* x, int dtype, int B, int F, int T, in
   }
   return EAT_OK;
 }
-
-}  // namespace
 
 extern "C" {
 
@@ -133,20 +89,6 @@ int eat_mean_len(const void* x, int dtype, float* out, int B, int F, int T, int 
   const dim3 grid(ceil_div(C, kMeanLanes), B), block(kMeanLanes, kMeanRows);
   if (dtype == EAT_BF16) mean_len_kernel<__nv_bfloat16><<<grid, block, 0, st>>>((const __nv_bfloat16*)x, out, F, T, C, t_valid);
   else mean_len_kernel<float><<<grid, block, 0, st>>>((const float*)x, out, F, T, C, t_valid);
-  EAT_CHECK_LAUNCH();
-  return EAT_OK;
-}
-
-int eat_ctx_pool_len(const void* x, int dtype, float* out, int B, int F, int T, int C, const int* t_valid,
-                     cudaStream_t st) {
-  if (int rc = len_check("ctx_pool_len", x, dtype, B, F, T, C, t_valid)) return rc;
-  const int V = dtype == EAT_BF16 ? 8 : 4;
-  if (C % V != 0) { eat_set_error("ctx_pool_len: channels must be a multiple of the vector width"); return EAT_ERR_ARG; }
-  if (B == 0) return EAT_OK;
-  if (out == nullptr) { eat_set_error("ctx_pool_len: out is required"); return EAT_ERR_ARG; }
-  const dim3 grid(ceil_div((F + T) * (C / V), 256), B);
-  if (dtype == EAT_BF16) ctx_pool_len_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, out, F, T, C, t_valid);
-  else ctx_pool_len_kernel<float><<<grid, 256, 0, st>>>((const float*)x, out, F, T, C, t_valid);
   EAT_CHECK_LAUNCH();
   return EAT_OK;
 }

@@ -1,14 +1,18 @@
 """DyReLU-B with M = 1..4 linear pieces (get_model(dyrelu_k=M)) against M = 2: the launches that take M, and whole
 AudioSetTrainer steps of dymn10 on 10 s clips.
 
-    python scripts/bench_dyrelu_k.py [--batch 128] [--rounds 7] [--steps 5] [--out gpu_out/dyrelu_k.json]
+    python scripts/bench_dyrelu_k.py [--batch 128] [--rounds 7] [--steps 5] [--baseline-lib PATH]
+                                     [--out gpu_out/dyrelu_k.json]
 
 Launches, fp32 storage, on three dymn10 10 s layer shapes: the eval depthwise conv with the DyReLU-B + CoordAtt epilogue
 (eat_dw_conv_fwd_dy_m; the 5x5 layer runs in the tile kernel), and the training-path DyReLU-B * CoordAtt forward and
-backward (eat_dy_act_fwd_m / eat_dy_act_bwd_m).  M = 2 goes through the same entry points, which hand it to the M = 2
-kernels.  Each launch is timed with CUDA events with the L2 flushed before it; M and M = 2 alternate round by round and
-the median is reported.  Algorithmic bytes come from the shapes: every tensor the launch must read or write once
-(activations, per-sample coefficient and attention tensors, gradients).  Trainer steps: eager AudioSetTrainer steps, the
+backward (eat_dy_act_fwd_m / eat_dy_act_bwd_m).  M = 2 goes through the same entry points.  Each launch is timed with
+CUDA events with the L2 flushed before it; M and M = 2 alternate round by round and the median is reported.  With
+--baseline-lib (another build of libeat_b200.so, for instance an earlier commit's) each launch alternates with the same
+launch and M of that build instead, and the outputs of the two builds are compared: bit for bit, except d(ca_f) and the
+coefficient gradients, which the backward sums with atomics in no fixed order (relative difference reported).
+Algorithmic bytes come from the shapes: every tensor the launch must read or write once (activations, per-sample
+coefficient and attention tensors, gradients).  Trainer steps: eager AudioSetTrainer steps, the
 four models alternating step by step in one process.  Prints the card, its power limit and maximum SM clock."""
 import argparse
 import contextlib
@@ -21,6 +25,7 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import efficientat_b200._lib as _lib  # noqa: E402
 from efficientat_b200._lib import lib  # noqa: E402
 
 HBM = 3.35e12       # H100 SXM data-sheet HBM3 bandwidth, bytes/s
@@ -34,7 +39,16 @@ def card():
     return q or torch.cuda.get_device_name()
 
 
-def kernels(B, rounds, L, st):
+def load(path):
+    """The C ABI of another build of the library, bound like lib()."""
+    saved, _lib.LIB_PATH = _lib.LIB_PATH, path
+    try:
+        return _lib._Lib()
+    finally:
+        _lib.LIB_PATH = saved
+
+
+def kernels(B, rounds, L, st, L0=None):
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 
     def one(fn):
@@ -54,47 +68,65 @@ def kernels(B, rounds, L, st):
         x = torch.randn(B, F, T, C, device="cuda")
         wt = torch.randn(B, kk, C, device="cuda") / k
         z, dp = torch.randn(B, Fo, To, C, device="cuda"), torch.randn(B, Fo, To, C, device="cuda")
-        out, du = torch.empty_like(z), torch.empty_like(z)
         sc = torch.rand(2, C, device="cuda") + 0.5
         ca_f, ca_t = torch.rand(B, Fo, C, device="cuda"), torch.rand(B, To, C, device="cuda")
-        dcaf, dcat = torch.zeros(B, Fo, C, device="cuda"), torch.empty(B, To, C, device="cuda")
         act = B * Fo * To * C * 4
         att = (B * Fo * C + B * To * C) * 4
 
-        def make(M):
-            theta = torch.rand(B, C, 2 * M, device="cuda")
-            lam = torch.tensor([1.0] * M + [0.5] * M, device="cuda")
-            init = torch.tensor([1.0] + [0.0] * (2 * M - 1), device="cuda")
+        def make(M, lib_):
+            theta, lam, init = coef[M]
+            out, du = torch.empty_like(z), torch.empty_like(z)
+            dcaf, dcat = torch.zeros(B, Fo, C, device="cuda"), torch.empty(B, To, C, device="cuda")
             dcoef = torch.zeros(B, C, 2 * M, device="cuda")
             P = (p(sc[0]), p(sc[1]), p(theta), p(lam), p(init), p(ca_f), p(ca_t))
             th = B * C * 2 * M * 4
             return {
                 "dw_eval": (x.numel() * 4 + act + th + att + B * kk * C * 4,
-                            lambda: L.dw_conv_fwd_dy_m(p(x), p(wt), kk * C, p(out), 0, B, F, T, C, k, s, 0, 0, 0, *P, M, 0, 0,
-                                                       st)),
-                "act_fwd": (2 * act + th + att, lambda: L.dy_act_fwd_m(p(z), p(out), 0, *P, M, B, Fo, To, C, st)),
+                            lambda: lib_.dw_conv_fwd_dy_m(p(x), p(wt), kk * C, p(out), 0, B, F, T, C, k, s, 0, 0, 0, *P, M,
+                                                          0, 0, st), dict(out=out)),
+                "act_fwd": (2 * act + th + att, lambda: lib_.dy_act_fwd_m(p(z), p(out), 0, *P, M, B, Fo, To, C, st),
+                            dict(out=out)),
                 "act_bwd": (3 * act + th + 2 * att + 2 * th,
-                            lambda: L.dy_act_bwd_m(p(dp), p(z), p(du), 0, *P, p(dcaf), p(dcat), p(dcoef), M, B, Fo, To, C,
-                                                   st)),
+                            lambda: lib_.dy_act_bwd_m(p(dp), p(z), p(du), 0, *P, p(dcaf), p(dcat), p(dcoef), M, B, Fo, To,
+                                                      C, st), dict(du=du, dcat=dcat, dcaf=dcaf, dcoef=dcoef)),
             }
-        base = make(2)
+        # the launches take raw pointers: theta, lam and init live as long as the shape's launches
+        coef = {M: (torch.rand(B, C, 2 * M, device="cuda"), torch.tensor([1.0] * M + [0.5] * M, device="cuda"),
+                    torch.tensor([1.0] + [0.0] * (2 * M - 1), device="cuda")) for M in (1, 2, 3, 4)}
+        base = make(2, L)
         for M in (1, 3, 4, 2):
-            cur = make(M)
-            for name, (nbytes, fn) in cur.items():
-                nb2, fn2 = base[name]
+            cur = make(M, L)
+            if L0 is not None:
+                base = make(M, L0)
+            for name, (nbytes, fn, outs) in cur.items():
+                nb2, fn2, outs2 = base[name]
                 fn(), fn2()                                   # warm-up: module load, shared-memory opt-in
+                same = {}
+                if L0 is not None:                            # one more launch each from zeroed accumulators
+                    for t in [*outs.values(), *outs2.values()]:
+                        t.zero_()
+                    fn(), fn2()
+                    torch.cuda.synchronize()
+                    for key, t in outs.items():
+                        t2 = outs2[key]
+                        same[key] = (bool(torch.equal(t, t2)) if key not in ("dcaf", "dcoef") else
+                                     ((t - t2).abs().max() / t2.abs().max().clamp_min(1e-30)).item())
                 tm, t2 = [], []
                 for _ in range(rounds):
                     tm.append(one(fn))
                     t2.append(one(fn2))
                 mm, m2 = sorted(tm)[rounds // 2], sorted(t2)[rounds // 2]
+                other = "M=2" if L0 is None else "baseline"
                 r = dict(shape=[B, F, T, C], k=k, stride=s, pieces=M, launch=name, bytes=nbytes, us=mm * 1e6,
-                         GBs=nbytes / mm / 1e9, hbm_share=nbytes / mm / HBM, m2_us=m2 * 1e6, m2_GBs=nb2 / m2 / 1e9,
-                         ratio=mm / m2)
+                         GBs=nbytes / mm / 1e9, hbm_share=nbytes / mm / HBM, ratio=mm / m2)
+                r["m2_us" if L0 is None else "baseline_us"] = m2 * 1e6
+                r["m2_GBs" if L0 is None else "baseline_GBs"] = nb2 / m2 / 1e9
+                if L0 is not None:
+                    r["vs_baseline"] = same
                 rows.append(r)
                 print(f"[{B},{F},{T},{C}] k{k} s{s} {name:8s} M={M} {mm * 1e6:8.1f} us {nbytes / mm / 1e9:6.0f} GB/s "
-                      f"({100 * nbytes / mm / HBM:4.1f} % of 3.35 TB/s) | M=2 {m2 * 1e6:8.1f} us | ratio {mm / m2:.2f}",
-                      flush=True)
+                      f"({100 * nbytes / mm / HBM:4.1f} % of 3.35 TB/s) | {other} {m2 * 1e6:8.1f} us | ratio {mm / m2:.2f}"
+                      + (f" | {same}" if same else ""), flush=True)
     return rows
 
 
@@ -134,6 +166,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=7)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--baseline-lib", default=None, help="another libeat_b200.so to alternate with and compare against")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -141,7 +174,8 @@ def main():
     dev = card()
     print("device:", dev, flush=True)
     L, st = lib(), torch.cuda.current_stream().cuda_stream
-    res = dict(device=dev, kernels=kernels(a.batch, a.rounds, L, st))
+    L0 = load(os.path.abspath(a.baseline_lib)) if a.baseline_lib else None
+    res = dict(device=dev, kernels=kernels(a.batch, a.rounds, L, st, L0))
     if a.steps > 0:
         res["trainer"] = steps(a.batch, a.steps, a.warmup)
     print(json.dumps(res))
