@@ -30,6 +30,7 @@ import torch
 import torch.nn.functional as Fn
 
 from efficientat_b200._lib import lib
+from tests.steady_util import dw_plan as _plan, out_hw as _out_hw
 from tests.util import bn_variance_check, report
 
 NONE, RELU, HS = 0, 1, 2
@@ -75,33 +76,8 @@ def _act(x, code):
     return torch.relu(x) if code == RELU else (Fn.hardswish(x) if code == HS else x)
 
 
-def _out_hw(F, T, k, s):
-    pad = (k - 1) // 2
-    return (F + 2 * pad - k) // s + 1, (T + 2 * pad - k) // s + 1
-
-
 def _ids(cases):
     return ["B{}_F{}_T{}_C{}_k{}_s{}".format(*c) for c in cases]
-
-
-def _plan(kind, dtype, B, F, T, C, k, s, per_sample=0):
-    """eat_dw_plan -> what the walk reaches: units per thread slot, segment rows vs rows, whether a thread's walk crosses
-    a sample boundary (flat plan, gy clipped below the CTAs that would give every slot one unit), partial last chunk"""
-    plan = (ctypes.c_int * 6)()
-    lib().dw_plan(kind, dtype, B, F, T, C, k, s, per_sample, ctypes.addressof(plan))
-    chunks, cvc, seg, groups, gy, P = list(plan)
-    if kind == 4:
-        return dict(chunks=chunks, tiles=seg, groups=groups, gy=gy)
-    Fo, To = _out_hw(F, T, k, s)
-    rows, cols = ((F + 1) // 2, T) if kind == 2 else (Fo, To)
-    V = 2 if (kind == 1 and k == 5) else (8 if dtype == BF16 else 4)
-    ppb = 128 // cvc
-    units1 = -(-cols // P) * -(-rows // seg)                   # units of one sample
-    slots = groups * ppb * (1 if per_sample else gy)
-    units = units1 * (1 if per_sample else B)
-    return dict(chunks=chunks, cvc=cvc, seg=seg, rows=rows, groups=groups, gy=gy, P=P, ppb=ppb, units1=units1,
-                gstep=slots, per_slot=units / slots, crosses=not per_sample and gy < -(-units // ppb),
-                partial=(C // V) % cvc != 0)
 
 
 def _ring_depth(dtype, C, k, s):

@@ -16,6 +16,7 @@ import torch
 import torch.nn.functional as Fn
 
 from efficientat_b200._lib import EatError, lib
+from tests import dymn_util as du
 from tests.util import report
 
 RELU, HS = 1, 2
@@ -509,14 +510,6 @@ def _dw_tables(B, C, k, g, pad=8):
     return buf, bstride, w
 
 
-def _conv_ps(x, w, k, s):
-    """x [B, F, T, C], w [B, k*k, C] -> per-sample depthwise conv, NHWC out"""
-    B, F, T, C = x.shape
-    wc = w.permute(0, 2, 1).reshape(B * C, 1, k, k)
-    y = Fn.conv2d(x.permute(0, 3, 1, 2).reshape(1, B * C, F, T), wc, None, s, (k - 1) // 2, 1, B * C)
-    return y.view(B, C, y.shape[2], y.shape[3]).permute(0, 2, 3, 1)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [F32, BF16], ids=["f32", "bf16"])
 @pytest.mark.parametrize("case", DW_CASES, ids=lambda c: "k{}_s{}_B{}".format(*c))
@@ -531,8 +524,8 @@ def test_dw_conv_dy_fwd_matches_fp64(case, dtype):
     d = _dy_inputs(B, Fo, To, C, F32, seed=k + s + B)
     rel = 1e-6 if dtype == F32 else BF16_REL
     wd = w.double()
-    conv = _conv_ps(x.double(), wd, k, s)
-    cmag = _conv_ps(x.double().abs(), wd.abs(), k, s)
+    conv = du.conv_ps(x.double(), wd, k, s)
+    cmag = du.conv_ps(x.double().abs(), wd.abs(), k, s)
     # eval form: BN affine + DyReLU-B + CoordAtt on the conv output
     out = torch.full((B, Fo, To, C), float("nan"), device="cuda").to(DT[dtype])
     L.dw_conv_fwd_dy(x.data_ptr(), buf.data_ptr(), bstride, out.data_ptr(), dtype, B, F, T, C, k, s, 0, 0, 0,
@@ -554,8 +547,8 @@ def test_dw_conv_dy_fwd_matches_fp64(case, dtype):
     L.dw_conv_fwd_dy(x.data_ptr(), buf.data_ptr(), bstride, out.data_ptr(), dtype, B, F, T, C, k, s, isc.data_ptr(),
                      ish.data_ptr(), HS, 0, 0, 0, 0, 0, 0, 0, stats[0].data_ptr(), stats[1].data_ptr(), st)
     xf = Fn.hardswish(x.double() * isc.double() + ish.double())
-    raw = _conv_ps(xf, wd, k, s)
-    rmag = _conv_ps(xf.abs(), wd.abs(), k, s)
+    raw = du.conv_ps(xf, wd, k, s)
+    rmag = du.conv_ps(xf.abs(), wd.abs(), k, s)
     w_t = _close_elem(out, raw, rel, 1e-5 * rmag + 1e-30, "dw_conv_fwd_dy training")
     # BatchNorm sums over B*Fo*To fp32 values (of the unrounded result): 1e-5 of sum |terms|
     w_s = _close_sum(stats[0], raw.sum((0, 1, 2)), rmag.sum((0, 1, 2)), 1e-5, "stat_sum")
@@ -586,9 +579,9 @@ def test_dw_conv_per_sample_backward_matches_fp64(case, dtype):
     assert bool((dw[B * C * kk:] == -777.0).all()), "dw_conv_wgrad wrote past the last sample's slice"
     xf = torch.relu(x.double() * isc.double() + ish.double())
     wv = torch.zeros(B, kk, C, dtype=torch.float64, device="cuda", requires_grad=True)
-    (_conv_ps(xf, wv, k, s) * dz.double()).sum().backward()
+    (du.conv_ps(xf, wv, k, s) * dz.double()).sum().backward()
     wabs = torch.zeros(B, kk, C, dtype=torch.float64, device="cuda", requires_grad=True)
-    (_conv_ps(xf.abs(), wabs, k, s) * dz.double().abs()).sum().backward()
+    (du.conv_ps(xf.abs(), wabs, k, s) * dz.double().abs()).sum().backward()
     to_ck = lambda t: t.permute(0, 2, 1).reshape(B, C * kk)                 # [B, k*k, C] -> [B, C*k*k] (dw [C,1,k,k])
     # a sum over Fo*To products per entry, fp32: 1e-5 of sum |terms|
     w_w = _close_sum(dw[: B * C * kk].view(B, C * kk), to_ck(wv.grad), to_ck(wabs.grad), 1e-5, "dw_conv_wgrad")
@@ -600,9 +593,9 @@ def test_dw_conv_per_sample_backward_matches_fp64(case, dtype):
         din = torch.full((B, F, T, C), float("nan"), device="cuda").to(DT[dtype])
         L.dw_conv_dgrad(dz.data_ptr(), buf.data_ptr(), bstride, _p(res), din.data_ptr(), dtype, B, F, T, C, k, s, st)
         xv = torch.zeros(B, F, T, C, dtype=torch.float64, device="cuda", requires_grad=True)
-        (_conv_ps(xv, w.double(), k, s) * dz.double()).sum().backward()
+        (du.conv_ps(xv, w.double(), k, s) * dz.double()).sum().backward()
         xa = torch.zeros(B, F, T, C, dtype=torch.float64, device="cuda", requires_grad=True)
-        (_conv_ps(xa, w.double().abs(), k, s) * dz.double().abs()).sum().backward()
+        (du.conv_ps(xa, w.double().abs(), k, s) * dz.double().abs()).sum().backward()
         ref, mag = xv.grad, xa.grad
         if res is not None:
             ref, mag = ref + res.double(), mag + res.double().abs()
@@ -652,94 +645,25 @@ def test_dymn_entry_points_reject_bad_arguments_before_any_launch():
 
 # ------------------------------------------------------------------------------------------------ training step at B = 5
 TRAIN_B, TRAIN_FRAMES = 5, 201
-WIDTH = {"dymn04": 0.4, "dymn10": 1.0}
+TRAIN_ROUTES, BOUNDS = du.TRAIN_ROUTES, du.BOUNDS
 _ORACLE = {}
 
 
 def _train_inputs():
-    from efficientat_b200.synth import synth_labels, synth_waveform
-    spec = synth_waveform(TRAIN_B, 128 * TRAIN_FRAMES, seed=21, std=0.7).view(TRAIN_B, 1, 128, TRAIN_FRAMES)
-    return spec, synth_labels(TRAIN_B, 527, seed=5)
+    return du.train_inputs(TRAIN_B, TRAIN_FRAMES)
 
 
 def _oracle(tag, temperature):
     """fp64 oracle training step (CPU, autograd): loss, logits, gradients, BatchNorm buffers after the step, eval
-    logits; cached per tag for the routes that share it"""
-    if tag in _ORACLE:
-        return _ORACLE[tag]
-    from oracle import net_oracle
-    from tests.util import build_model
-    model = build_model(tag)
-    params = {k for k, _ in model.named_parameters()}
-    sd0 = {k: (v.double() if v.is_floating_point() else v).clone() for k, v in model.state_dict().items()}
-    spec, y = _train_inputs()
-    # eval: the golden state's BatchNorm buffers were calibrated on other clips, and on these the eval-mode network
-    # saturates (logits ~1e10); calibrate them on this batch as tests/golden/make_golden.py does (one training-mode pass
-    # with momentum 1)
-    cal = {k: v.clone() for k, v in sd0.items()}
-    mom = net_oracle.BN_MOM
-    try:
-        net_oracle.BN_MOM = 1.0
-        with torch.no_grad():
-            net_oracle.dymn_forward(cal, spec.double(), width_mult=WIDTH[tag], training=True, temperature=temperature)
-    finally:
-        net_oracle.BN_MOM = mom
-    cal = {k: v for k, v in cal.items() if k.endswith(("running_mean", "running_var"))}
-    with torch.no_grad():
-        ev, _ = net_oracle.dymn_forward({**sd0, **cal}, spec.double(), width_mult=WIDTH[tag], temperature=temperature)
-    sd = {k: v.clone() for k, v in sd0.items()}
-    for k in params:
-        sd[k].requires_grad_(True)
-    logits, _ = net_oracle.dymn_forward(sd, spec.double(), width_mult=WIDTH[tag], training=True, temperature=temperature)
-    loss = Fn.binary_cross_entropy_with_logits(logits, y.double())
-    loss.backward()
-    out = dict(loss=loss.item(), logits=logits.detach(), eval_logits=ev, cal=cal,
-               grads={k: sd[k].grad.detach() for k in params},
-               buffers={k: v.detach() for k, v in sd.items() if k.endswith(("running_mean", "running_var"))})
-    _ORACLE[tag] = out
-    return out
+    logits (the golden state's BatchNorm buffers were calibrated on other clips, and on these the eval-mode network
+    saturates, logits ~1e10: calibrated on this batch); cached per tag for the routes that share it"""
+    if tag not in _ORACLE:
+        _ORACLE[tag] = du.oracle_step(tag, temperature, *_train_inputs())
+    return _ORACLE[tag]
 
 
 def _engine_step(tag, precision, gemm, dyn_tma_min_rps=None):
-    from tests.util import build_model
-    spec, y = _train_inputs()
-    model = build_model(tag, precision=precision).cuda().train()
-    eng = model.engine()
-    eng.gemm_impl = gemm
-    if dyn_tma_min_rps is not None:
-        eng.dyn_tma_min_rps = dyn_tma_min_rps
-    model.classifier[4].p = 0.0
-    eng.dropout_p = 0.0
-    logits, _ = model(spec.cuda())
-    loss = Fn.binary_cross_entropy_with_logits(logits, y.cuda())
-    loss.backward()
-    return model, loss.item(), logits.detach().double().cpu()
-
-
-def _grad_errors(model, ref):
-    """per-tensor relative L2 of every gradient against the oracle; tensors whose fp64 gradient is analytically zero
-    (BatchNorm biases whose constant shift the next training-mode BatchNorm removes: below 1e-9 of the whole gradient's
-    norm) are measured against the whole gradient's norm instead"""
-    total = torch.sqrt(sum((g * g).sum() for g in ref["grads"].values())).item()
-    rel, zero, norm = {}, {}, {}
-    for n, p in model.named_parameters():
-        g = p.grad.detach().double().cpu()
-        r = ref["grads"][n]
-        e = (g - r).norm().item()
-        if r.norm().item() <= 1e-9 * total:
-            zero[n] = e / total
-        else:
-            rel[n] = e / r.norm().item()
-            norm[n] = abs(g.norm().item() - r.norm().item()) / r.norm().item()
-    return rel, zero, norm
-
-
-# route -> (gemm, dyn_tma_min_rps) and the bounds on every gradient tensor: (relative L2, relative error of the norm) for
-# the attention-logit layers (`*.residuals.0.*`) and for all other tensors, and the logits' max-abs error
-TRAIN_ROUTES = {"simt": ("simt", None), "auto_tma": ("auto", 0), "auto_reg": ("auto", 10 ** 9)}
-BOUNDS = {"simt": dict(res=(2e-2, 1e-2), other=(1e-2, 2e-3), logits=5e-5),
-          "auto_tma": dict(res=(0.25, 0.2), other=(0.15, 3e-2), logits=5e-4),
-          "auto_reg": dict(res=(0.25, 0.2), other=(0.15, 3e-2), logits=5e-4)}
+    return du.engine_step(tag, precision, gemm, *_train_inputs(), dyn_tma_min_rps=dyn_tma_min_rps)
 
 
 @pytest.mark.gpu
@@ -761,34 +685,9 @@ def test_dymn_train_step_b5_matches_fp64_oracle(tag, route):
     worst figure.  The one analytically-zero gradient (a BatchNorm bias whose shift the next training-mode BatchNorm
     removes; fp64 gives 1e-9 of the gradient norm) is bounded against the whole gradient's norm (measured 1.5e-9)."""
     gemm, min_rps = TRAIN_ROUTES[route]
-    from tests.util import build_model
-    temperature = float(build_model(tag).layers[0].depth_conv.temperature)
-    ref = _oracle(tag, temperature)
+    ref = _oracle(tag, du.temperature(tag))
     model, loss, logits = _engine_step(tag, "fp32", gemm, min_rps)
-    lerr = (logits - ref["logits"]).abs().max().item()
-    rel, zero, norm = _grad_errors(model, ref)
-    res_rel = max(v for n, v in rel.items() if ".residuals." in n)
-    oth_rel = max(v for n, v in rel.items() if ".residuals." not in n)
-    worst_oth = max((v, n) for n, v in rel.items() if ".residuals." not in n)[1]
-    buf = model.state_dict()
-    berr = max(((buf[k].double().cpu() - v).abs().max().item() / max(1.0, v.abs().max().item()))
-               for k, v in ref["buffers"].items())
-    report(f"[parity] {tag} B={TRAIN_B} train route={route}: loss {abs(loss - ref['loss']):.2e}, logits {lerr:.2e}, "
-           f"grad rel-L2 max {oth_rel:.2e} ({worst_oth}), attention-logit layers {res_rel:.2e}, "
-           f"analytically-zero tensors {max(zero.values(), default=0.0):.2e} of the gradient norm ({len(zero)}), "
-           f"BatchNorm buffers {berr:.2e}; grad-norm rel err max {max(v for n, v in norm.items() if '.residuals.' not in n):.2e}"
-           f" (attention-logit layers {max(v for n, v in norm.items() if '.residuals.' in n):.2e})")
-    bd = BOUNDS[route]
-    assert abs(loss - ref["loss"]) < 1e-5 * max(1.0, abs(ref["loss"])), (loss, ref["loss"])
-    assert lerr < bd["logits"], lerr
-    assert berr < 1e-5, berr                                  # running statistics, relative to max(1, |value|)
-    bad = []
-    for n, v in rel.items():
-        brel, bnorm = bd["res" if ".residuals." in n else "other"]
-        if v > brel or norm[n] > bnorm:
-            bad.append(f"{n}: relative L2 {v:.2e} (bound {brel:.0e}), norm {norm[n]:.2e} (bound {bnorm:.0e})")
-    assert not bad, "\n".join(bad)
-    assert max(zero.values(), default=0.0) < 1e-7
+    du.check_train_step(f"{tag} B={TRAIN_B} train", route, model, loss, logits, ref)
 
 
 @pytest.mark.gpu
@@ -796,8 +695,7 @@ def test_dymn_train_step_b5_matches_fp64_oracle(tag, route):
 def test_dymn_eval_b5_matches_fp64_oracle(tag):
     """eval forward at B = 5, exact-fp32 route: logits within 1e-4 of the fp64 oracle"""
     from tests.util import build_model
-    temperature = float(build_model(tag).layers[0].depth_conv.temperature)
-    ref = _oracle(tag, temperature)
+    ref = _oracle(tag, du.temperature(tag))
     spec, _ = _train_inputs()
     model = build_model(tag)
     with torch.no_grad():
@@ -823,12 +721,10 @@ def test_dymn_bf16_train_step_b5_against_fp64_oracle():
     3.4e-2; from the out_c conv on, every tensor 0.2-0.6 (median 0.42, max 1.1 / 1.6; attention-logit layers up to 5.2).
     The error appears at the last BatchNorm's backward and stays level through the network instead of growing in any
     one DyMN layer: amplified rounding, not a kernel defect (the kernels alone pass the bf16 cases above)."""
-    from tests.util import build_model
     tag = "dymn04"
-    temperature = float(build_model(tag).layers[0].depth_conv.temperature)
-    ref = _oracle(tag, temperature)
+    ref = _oracle(tag, du.temperature(tag))
     model, loss, logits = _engine_step(tag, "bf16", "auto")
-    rel, zero, _ = _grad_errors(model, ref)
+    rel, zero, _ = du.grad_errors(du.grads_of(model), ref)
     names = [n for n, _ in model.named_parameters()]
     g = torch.cat([dict(model.named_parameters())[n].grad.detach().double().cpu().flatten() for n in names])
     r = torch.cat([ref["grads"][n].flatten() for n in names])

@@ -44,16 +44,11 @@ import pytest
 import torch
 
 from efficientat_b200._lib import lib
+from tests.steady_util import (C_PROD, HS, RELU, SMS, SUM_ULPS, U, check_prod as _check_prod, chunks as _chunks,
+                               dc as _dc, fwd_operands as _fwd_operands, tma_plan as _tma_plan, ulps as _ulps,
+                               wgrad_ref as _wgrad_ref)
 from tests.util import bn_variance_check, report
 
-RELU, HS = 1, 2
-U = 2.0 ** -24
-SMS = 132                         # H100 SXM
-# long-sum bound in units of 2^-24 * sum |terms| (measured on an H100 80GB HBM3 at 700 W: <= 20 without products)
-SUM_ULPS = 64
-# the bf16x3 products and the tensor core's fp32 accumulation over one flush window of the weight-gradient kernels, of
-# sum |terms| (measured <= 1.7e-5); planted defects sit >= 20x above the bound
-C_PROD = 1e-4
 TOL_OUT = 2e-4                    # dX / dp of the fused kernels, of the tensor's max
 EPS = 1e-3                        # nn.BatchNorm2d(eps=1e-3)
 GIB = 2.0 ** 30
@@ -155,12 +150,6 @@ def _reduce_cases():
 
 
 # ------------------------------------------------------------------------------------------------ planners
-def _tma_plan(M, N, K, rps=0):
-    pl = (ctypes.c_int * 5)()
-    lib().pw_tma_plan(M, N, K, rps, 1, SMS, ctypes.addressof(pl))
-    return dict(zip(("BN", "n_tiles", "m_tiles", "grid", "per_cta"), list(pl)))
-
-
 def _wg_plan(M, N, K, rps=0, per_sample=0):
     pl = (ctypes.c_int * 6)()
     lib().pw_wgrad_plan(M, N, K, rps, per_sample, SMS, ctypes.addressof(pl))
@@ -209,44 +198,16 @@ def test_cases_reach_the_steady_state():
 
 
 # ------------------------------------------------------------------------------------------------ helpers
-def _dc(shape, g, device="cuda"):
-    """4 + 0.25 randn: positive, mean >> std"""
-    return torch.randn(*shape, device=device, generator=g).mul_(0.25).add_(4.0)
-
-
-def _ulps(got, ref, mag):
-    """worst |got - ref| in units of 2^-24 mag"""
-    return ((got.double() - ref).abs() / (U * mag + 1e-300)).max().item()
-
-
 def _check(got, ref, mag, what):
     u = _ulps(got, ref, mag)
     assert u <= SUM_ULPS, f"{what}: error {u:.1f} x 2^-24 sum|terms| (bound {SUM_ULPS})"
     return u
 
 
-def _chunks(M, cols, budget=1 << 25):
-    step = max(128, budget // max(cols, 1))
-    return [(m, min(M, m + step)) for m in range(0, M, step)]
-
-
 def _peak(what):
     peak = torch.cuda.max_memory_allocated() / GIB
     report(f"[kernel] pw {what}: peak device memory {peak:.2f} GiB")
     assert peak < 8, f"{what}: peak device memory {peak:.2f} GiB"
-
-
-def _fwd_operands(M, N, K, rps, g, dyn_k=4):
-    """A [M, K] with a constant first column, W [N, K] (dyn: [dyn_k, N, K] + softmax attention): column n of C has
-    mean r_n * s_n and std s_n, r_n from 4 to 24"""
-    A = torch.randn(M, K, device="cuda", generator=g)
-    A[:, 0] = 1.0
-    nw = dyn_k if rps else 1
-    W = torch.randn(nw, N, K, device="cuda", generator=g) / K ** 0.5
-    s = W[0, :, 1:].norm(dim=1)
-    W[:, :, 0] = torch.linspace(4.0, 24.0, N, device="cuda") * s
-    att = torch.softmax(torch.randn(M // rps, dyn_k, device="cuda", generator=g), 1) if rps else None
-    return A, (W if rps else W[0].contiguous()), att
 
 
 # ------------------------------------------------------------------------------------------------ forward statistics
@@ -321,41 +282,6 @@ def test_forward_statistics_bf16_storage(case):
 
 
 # ------------------------------------------------------------------------------------------------ weight gradients
-def _xf(x, sc, act, gate, rps, m0):
-    a = x.double()
-    if sc is not None:
-        a = a * sc[0].double() + sc[1].double()
-        a = a.clamp_min(0) if act == RELU else (a * (a + 3).clamp(0, 6) / 6 if act == HS else a)
-    if gate is not None:
-        rows = torch.arange(m0, m0 + x.shape[0], device=x.device) // rps
-        a = a * gate.double()[rows]
-    return a
-
-
-def _wgrad_ref(G, X, sc, act, gate, rps, per_sample):
-    """fp64 dW ([1, N, K], per sample [B, N, K]) and sum |g| |xf| per entry, in chunks"""
-    M, N = G.shape
-    K = X.shape[1]
-    nb = M // rps if per_sample else 1
-    ref = torch.zeros(nb, N, K, device="cuda", dtype=torch.float64)
-    mag = torch.zeros_like(ref)
-    spans = [(b * rps, (b + 1) * rps) for b in range(nb)] if per_sample else _chunks(M, N + K)
-    for m0, m1 in spans:
-        gg, xx = G[m0:m1].double(), _xf(X[m0:m1], sc, act, gate, rps, m0)
-        i = m0 // rps if per_sample else 0
-        ref[i] += gg.t() @ xx
-        mag[i] += gg.abs().t() @ xx.abs()
-        del gg, xx
-    return ref, mag
-
-
-def _check_prod(got, ref, mag, what, c_prod=C_PROD):
-    """|got - ref| <= (c_prod + SUM_ULPS * 2^-24) * mag per entry; returns the worst error in units of 2^-24 mag"""
-    u = ((got.double() - ref).abs() / (U * mag + 1e-300)).max().item()
-    assert u <= c_prod / U + SUM_ULPS, f"{what}: error {u:.0f} x 2^-24 sum|terms| (bound {c_prod / U + SUM_ULPS:.0f})"
-    return u
-
-
 WGRAD_XF = [("none", None), ("bn_relu", RELU), ("bn_hs", HS), ("gate", "gate")]
 
 
